@@ -262,6 +262,25 @@ int gs_pack_frame(GsContext* ctx, int32_t H, int32_t W, const float* color, cons
                   float* neg_depth, uint32_t* minmax_state, gs_stream_t stream);
 int gs_minmax_read(GsContext* ctx, uint32_t* minmax_state, float* minmax2, gs_stream_t stream);
 
+/* Depth colour mapping of a clip: `depthlist = [colorize(depth) for depth in depthlist]` (luciddreamer.py:267,
+ * utils/depth.py:7-62 with cmap 'jet'), for F frames in one fixed sequence of launches.  Per frame, over the valid pixels
+ * (value != invalid_val):
+ *   vmin, vmax = np.percentile(valid, 2), np.percentile(valid, 98)   evaluated as numpy does for float32 input
+ *                (float32 index (n-1) * float32(q/100), float32 lerp), from exact order statistics (radix select)
+ *   x = (value - vmin) / (vmax - vmin)  (IEEE float32) if vmin != vmax, else 0
+ *   rgba[y][x] = lut_rgba[clamp(trunc(x * 256), 0, 255)] (x < 0 -> entry 0, x > 1 -> entry 255); invalid pixels get
+ *                background_rgba (bytes R, G, B, A in memory order, i.e. R | G << 8 | B << 16 | A << 24)
+ * The result is bit-identical to the host restatement (luciddreamer_b200.video.colorize) on the same float32 frame.
+ * A frame without a valid pixel (where np.percentile raises) is all background and gets NaN for its (vmin, vmax).
+ * -0.0 and +0.0 count as one value; NaN / inf depths are outside the contract (every output byte is still written).
+ *   value: [F,H,W] f32 device; lut_rgba: [256,4] u8 device; rgba: [F,H,W,4] u8 device; all 4-byte aligned
+ *   vminmax: [F,2] f32 device, or NULL;  scratch: gs_colorize_scratch_bytes(F) bytes, 16-byte aligned
+ * Pure stream work (capturable in a CUDA graph).  ctx is not used and may be NULL. */
+size_t gs_colorize_scratch_bytes(int32_t F);
+int gs_colorize_depth(GsContext* ctx, int32_t F, int32_t H, int32_t W, const float* value, float invalid_val,
+                      const uint8_t* lut_rgba, uint32_t background_rgba, void* scratch, size_t scratch_bytes,
+                      uint8_t* rgba, float* vminmax, gs_stream_t stream);
+
 /* "Next" row (SURVEY.md 8f-3): simple_knn.distCUDA2 (submodules/simple-knn/spatial.cu:15-26 over SimpleKNN::knn,
  * simple_knn.cu:185-221): mean_dist2[i] = mean of the squared distances from point i to its 3 nearest other points
  * (exact search; bit-identical to the reference, incl. duplicates and P < 4).  points: [P,3] f32 device;

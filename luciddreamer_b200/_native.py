@@ -87,6 +87,9 @@ SYMBOLS = [
     ("gs_pack_frame", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p]),
     ("gs_minmax_read", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("gs_colorize_scratch_bytes", C.c_size_t, [C.c_int32]),
+    ("gs_colorize_depth", C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_float, C.c_void_p,
+                                    C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("gs_knn_scratch_bytes", C.c_size_t, [C.c_int32]),
     ("gs_knn_mean_dist2", C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("gs_densify_stats", C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -719,6 +719,29 @@ int gs_minmax_read(GsContext* ctx, uint32_t* minmax_state, float* minmax2, gs_st
     return GS_OK;
 }
 
+size_t gs_colorize_scratch_bytes(int32_t F) { return F > 0 ? gs_colorize_scratch_bytes_impl(F) : 0; }
+
+int gs_colorize_depth(GsContext* ctx, int32_t F, int32_t H, int32_t W, const float* value, float invalid_val,
+                      const uint8_t* lut_rgba, uint32_t background_rgba, void* scratch, size_t scratch_bytes,
+                      uint8_t* rgba, float* vminmax, gs_stream_t stream) {
+    (void)ctx;
+    if (F <= 0 || H <= 0 || W <= 0) return fail(GS_EINVAL, "bad sizes F=%d H=%d W=%d", F, H, W);
+    if ((int64_t)H * W > 0x7fffffffLL) return fail(GS_EINVAL, "frame too large");
+    if (!value || !lut_rgba || !scratch || !rgba) return fail(GS_EINVAL, "NULL argument");
+    if ((reinterpret_cast<uintptr_t>(value) | reinterpret_cast<uintptr_t>(lut_rgba) | reinterpret_cast<uintptr_t>(rgba) |
+         reinterpret_cast<uintptr_t>(vminmax)) & 3)
+        return fail(GS_EINVAL, "value, lut_rgba, rgba and vminmax must be 4-byte aligned");
+    if (reinterpret_cast<uintptr_t>(scratch) & 15) return fail(GS_EINVAL, "scratch must be 16-byte aligned");
+    const size_t need = gs_colorize_scratch_bytes(F);
+    if (scratch_bytes < need) return fail(GS_EINVAL, "scratch too small: %zu < %zu bytes", scratch_bytes, need);
+    const int rc = gs_launch_colorize(F, H, W, value, invalid_val, reinterpret_cast<const uint32_t*>(lut_rgba),
+                                      background_rgba, scratch, reinterpret_cast<uint32_t*>(rgba), vminmax,
+                                      (cudaStream_t)stream);
+    cudaError_t e = rc != 0 ? (cudaError_t)rc : cudaPeekAtLastError();
+    if (e != cudaSuccess) return fail(GS_ECUDA, "colorize launch: %s", cudaGetErrorString(e));
+    return GS_OK;
+}
+
 size_t gs_knn_scratch_bytes(int32_t P) { return P > 0 ? gs_knn_scratch_bytes_impl(P) : 256; }
 
 int gs_knn_mean_dist2(GsContext* ctx, int32_t P, const float* points, void* scratch, float* mean_dist2, gs_stream_t stream) {

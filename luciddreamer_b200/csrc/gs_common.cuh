@@ -398,6 +398,9 @@ int gs_launch_gaussian_adam(GsAdamArgs a, cudaStream_t s);
 void gs_launch_pack_frame(int N, const float* color, const float* depth, uint8_t* rgb8, float* depth_out, unsigned* minmax,
                           cudaStream_t s);
 void gs_launch_minmax_decode(unsigned* mm, float* out2, cudaStream_t s);
+size_t gs_colorize_scratch_bytes_impl(int F);
+int gs_launch_colorize(int F, int H, int W, const float* value, float invalid_val, const uint32_t* lut, uint32_t bg,
+                       void* scratch, uint32_t* rgba, float* vminmax, cudaStream_t s);
 size_t gs_knn_scratch_bytes_impl(int P);
 int gs_launch_knn(int P, const float* points, void* scratch, float* out, cudaStream_t s);
 void gs_launch_densify_stats(int P, const int* radii, const float* dm2, float* accum, float* denom, float* max_radii,

@@ -7,9 +7,11 @@ host memory ONCE.  The reference pays two blocking float D2H copies (16 B/pixel)
 
 `load_json` restates utils/camera.py:24-52 (the preset camera files under cameras/*.json), including its
 MiniCam(W, H, FoVx, FoVy, ...) argument-order quirk (see synthetic.make_camera).
-`colorize` restates utils/depth.py:7-62 for the host side of the depth video."""
+`colorize` restates utils/depth.py:7-62 for the host side of the depth video; `colorize_frames` does the same for a whole
+clip on the device (gs_colorize_depth), and `render_video_frames(..., depth_rgba=True)` returns the coloured clip."""
 from __future__ import annotations
 
+import inspect
 import json
 from typing import Optional, Sequence
 
@@ -44,12 +46,48 @@ def pack_frame(color: torch.Tensor, depth: Optional[torch.Tensor], rgb8: torch.T
                                       R._raw_stream(idx)))
 
 
-def render_video_frames(params: dict, settings_list: Sequence, rank: int = 0, world: int = 1, with_depth: bool = True):
+def colorize_frames(neg_depth: torch.Tensor):
+    """`colorize` for every frame of a clip, on the device (gs_colorize_depth), on the current stream without a host sync.
+
+    neg_depth: [F,H,W] float32 CUDA tensor (e.g. the depths render_video_frames packs).  Returns (rgba uint8 [F,H,W,4],
+    vminmax float32 [F,2]) on the same device: frame k of `rgba` is bit-identical to `colorize(neg_depth[k])`, and
+    vminmax[k] holds its (2nd, 98th) percentiles.  A frame without a valid pixel (where `colorize` raises) comes out as
+    background with NaN percentiles.  invalid_val and the background colour are `colorize`'s defaults."""
+    if not isinstance(neg_depth, torch.Tensor) or neg_depth.dtype != torch.float32 or neg_depth.dim() != 3:
+        raise ValueError("colorize_frames: expected a float32 [F,H,W] tensor, got "
+                         f"{getattr(neg_depth, 'dtype', type(neg_depth))} {tuple(getattr(neg_depth, 'shape', ()))}")
+    if not neg_depth.is_cuda:
+        raise RuntimeError("colorize_frames: CUDA tensors only (no CPU fallback)")
+    value = neg_depth.contiguous()
+    F, H, W = value.shape
+    dev = value.device
+    rgba = torch.empty((F, H, W, 4), dtype=torch.uint8, device=dev)
+    vminmax = torch.empty((F, 2), dtype=torch.float32, device=dev)
+    if value.numel() == 0:
+        return rgba, vminmax.fill_(float("nan"))
+    idx = dev.index
+    lut = _device_lut(dev)
+    L = N.lib()
+    scratch = torch.empty(L.gs_colorize_scratch_bytes(F), dtype=torch.uint8, device=dev)
+    with R._guard(idx):
+        N.check(L.gs_colorize_depth(R._ctx(idx), F, H, W, value.data_ptr(), float(_INVALID_VAL), lut.data_ptr(),
+                                    _BACKGROUND_RGBA, scratch.data_ptr(), scratch.numel(), rgba.data_ptr(),
+                                    vminmax.data_ptr(), R._raw_stream(idx)))
+    return rgba, vminmax
+
+
+def render_video_frames(params: dict, settings_list: Sequence, rank: int = 0, world: int = 1, with_depth: bool = True,
+                        depth_rgba: bool = False):
     """Renders this rank's share (views rank, rank+world, ...) of `settings_list`.
 
     params: dict(means3D, shs, opacities, scales, rotations) of CUDA tensors (activated values, as render() passes them).
     Returns (frames uint8 [F,H,W,3] numpy, depths float32 [F,H,W] numpy or None, dmin, dmax, view_indices) with the
-    semantics of framelist / depthlist / dmin / dmax in luciddreamer.py:241-262.  One host copy for the whole clip."""
+    semantics of framelist / depthlist / dmin / dmax in luciddreamer.py:241-262.  One host copy for the whole clip.
+    depth_rgba=True: the depths are colour-mapped on the device before that copy (`colorize_frames`, one call for the
+    clip), and the second element is the coloured depth clip, uint8 [F,H,W,4] -- what luciddreamer.py:267 makes of
+    depthlist."""
+    if depth_rgba and not with_depth:
+        raise ValueError("render_video_frames: depth_rgba=True needs with_depth=True")
     from .multiview import shard_views
     views = shard_views(len(settings_list), rank, world)
     dev = params["means3D"].device
@@ -77,8 +115,13 @@ def render_video_frames(params: dict, settings_list: Sequence, rank: int = 0, wo
         idx = dev.index
         with R._guard(idx):
             N.check(N.lib().gs_minmax_read(R._ctx(idx), state.data_ptr(), mm.data_ptr(), R._raw_stream(idx)))
-        h_d = torch.empty((F, H, W), dtype=torch.float32, pin_memory=True)
-        h_d.copy_(negd, non_blocking=True)
+        if depth_rgba:
+            d_rgba, _ = colorize_frames(negd)
+            h_d = torch.empty((F, H, W, 4), dtype=torch.uint8, pin_memory=True)
+            h_d.copy_(d_rgba, non_blocking=True)
+        else:
+            h_d = torch.empty((F, H, W), dtype=torch.float32, pin_memory=True)
+            h_d.copy_(negd, non_blocking=True)
         h_mm = torch.empty(2, dtype=torch.float32, pin_memory=True)
         h_mm.copy_(mm, non_blocking=True)
     torch.cuda.current_stream(dev).synchronize()
@@ -138,3 +181,21 @@ def colorize(value, vmin=None, vmax=None, invalid_val=-99, invalid_mask=None, ba
     img = jet_lut()[idx]
     img[invalid_mask] = background_color
     return img
+
+
+# ------------------------------------------------------------------------------------------------ device side: colorize
+_COLORIZE_DEFAULTS = inspect.signature(colorize).parameters
+_INVALID_VAL = _COLORIZE_DEFAULTS["invalid_val"].default
+_BACKGROUND_RGBA = int.from_bytes(bytes(_COLORIZE_DEFAULTS["background_color"].default), "little")   # R | G<<8 | B<<16 | A<<24
+_LUT_ON_DEVICE = {}
+
+
+def _device_lut(dev: torch.device) -> torch.Tensor:
+    """jet_lut() as a [256,4] uint8 tensor on `dev`, copied once per device."""
+    t = _LUT_ON_DEVICE.get(dev.index)
+    if t is None:
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("colorize_frames: call it once on this device before capturing a CUDA graph "
+                               "(the colour table is copied to the device on first use)")
+        t = _LUT_ON_DEVICE[dev.index] = torch.from_numpy(jet_lut().copy()).to(dev)
+    return t
