@@ -179,6 +179,7 @@ int gs_context_create(int device, GsContext** out) {
     gs_grad_write_init();
     gs_preprocess_init();
     if (const char* e = getenv("GS_BLEND_VARIANT")) g_gs_blend_variant = atoi(e);
+    if (const char* e = getenv("GS_BLEND_BWD")) g_gs_blend_bwd = atoi(e);
     cudaError_t e = cudaHostAlloc((void**)&c->slots, sizeof(GsDevStatus) * (kSlots + kGraphSlots),
                                 cudaHostAllocMapped | cudaHostAllocPortable);
     if (e != cudaSuccess) {

@@ -30,149 +30,16 @@
 //    1/(1-alpha) is a single MUFU.RCP (the gradient tolerance is 1e-3 relative).
 // k_tile_partials (deterministic backward, opt-in) is k_blend_bwd with the reductions replaced by plain stores of the
 //   same nine values per list position; gs_det_bwd.cu sums them per Gaussian in a fixed order.
+// The default backward pass is gs_blend_bwd.cu (same arithmetic, a transposed shared-memory reduction instead of the
+// shuffle butterfly, bit-identical sums); the kernels here stay selectable with GS_BLEND_BWD=0.
 #include <cstdlib>
 
-#include "gs_common.cuh"
+#include "gs_blend.cuh"
 
 namespace {
 
 constexpr int kBatch = 128;           // splats staged per round
 constexpr int kWords = kBatch / 32;
-
-// Two geometries, chosen per launch by the number of tiles (gs_launch_blend_*):
-//   NH = 2  a warp owns a 16x8 block, a thread FOUR pixels (two float2 pairs); 2 warps (64 threads) per tile
-//   NH = 1  a warp owns a 16x4 strip, a thread TWO pixels (one pair); 4 warps (128 threads) per tile -- twice the warps
-//           for images with few tiles (512x512: 1024 tiles would leave the SMs at 14 resident warps), finer culling
-template <int NH> struct Geo {
-    static constexpr int RW = 4 * NH;             // pixel rows per warp
-    static constexpr int NW = 16 / RW;            // warps per tile
-    static constexpr int NT = 32 * NW;            // threads per CTA
-    static constexpr int NQ = 2 * NH;             // pixels per thread
-};
-
-struct __align__(16) SRec {           // shared-memory copy of a splat record
-    float4 a;                         // x, y, A2 = -0.5 log2e conic_a, B2 = -log2e conic_b
-    float4 b;                         // C2 = -0.5 log2e conic_c, opacity, r, g
-    float2 c;                         // b, depth
-    uint32_t id;
-    uint32_t generic;                 // != 0: not eligible for the fast path
-};
-
-constexpr float kHalfLog2e = -0.5f * 1.4426950408889634f;     // staged conic scale (see stage_batch)
-constexpr float kUnscale = -2.0f * 0.6931471805599453f;       // back to the conic for the flush of the backward pass
-constexpr float kAlphaMin = 1.0f / 255.0f;
-constexpr float kBand = 1e-7f;
-constexpr float kNegInf = -__builtin_huge_valf();
-
-// ---- FP32 pairs: two pixels per call, one FFMA / FMUL / FADD per pixel (sm_90 has no packed FP32 instructions).
-// The _rn intrinsics round every product and sum on its own: the compiler may not contract a mul2 + add2 into an fma.
-__device__ __forceinline__ float2 fma2(const float2 a, const float2 b, const float2 c) {
-    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
-}
-__device__ __forceinline__ float2 mul2(const float2 a, const float2 b) {
-    return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
-}
-__device__ __forceinline__ float2 add2(const float2 a, const float2 b) {
-    return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
-}
-__device__ __forceinline__ float2 bc(const float s) { return make_float2(s, s); }
-__device__ __forceinline__ float ex2_approx(const float x) {
-    float y;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
-__device__ __forceinline__ float rcp_approx(const float x) {
-    float y;
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
-
-// NW-bit mask: which of the tile's 16 x RW pixel strips the splat can touch
-template <int NH>
-__device__ __forceinline__ uint32_t strip_mask(const float4 a, const float4 b, const float thr, int tx0, int ty0) {
-    uint32_t m = 0;
-#pragma unroll
-    for (int w = 0; w < Geo<NH>::NW; w++) {
-        const float x0 = (float)tx0, y0 = (float)(ty0 + Geo<NH>::RW * w);
-        if (gs_box_hit(a.x, a.y, a.z, a.w, b.x, thr, x0, y0, x0 + 15.f, y0 + (float)(Geo<NH>::RW - 1))) m |= 1u << w;
-    }
-    return m;
-}
-
-// Stages up to kBatch splats into shared memory and publishes the per-strip hit masks.
-// slot j of the batch holds list position pos(j).  Mask words are bit-REVERSED (slot 32k+i -> bit 31-i) so the
-// traversal finds the next slot with one FLO (count-leading-zeros).  All threads must call.
-template <int NH, typename PosFn>
-__device__ __forceinline__ void stage_batch(SRec* sRec, uint32_t (*sMask)[kWords], const uint32_t* __restrict__ list,
-                                            const float4* __restrict__ rec, uint32_t beg, int cnt, int tx0, int ty0,
-                                            PosFn pos_of) {
-    constexpr int NW = Geo<NH>::NW, NT = Geo<NH>::NT;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-#pragma unroll
-    for (int h = 0; h < kBatch / NT; h++) {
-        const int j = tid + h * NT;
-        uint32_t m = 0;
-        if (j < cnt) {
-            const uint32_t id = list[beg + pos_of(j)];
-            const float4* r = rec + (size_t)GS_REC_V4 * id;
-            const float4 a = __ldg(r), b = __ldg(r + 1), c = __ldg(r + 2);
-            // the conic is staged pre-multiplied for the exponent in base 2:
-            //   log2(e) * power = A2 dx dx + C2 dy dy + B2 dx dy,  A2 = -0.5 log2e A, C2 = -0.5 log2e C, B2 = -log2e B
-            SRec s; s.a = make_float4(a.x, a.y, a.z * kHalfLog2e, a.w * (2.f * kHalfLog2e));
-            s.b = make_float4(b.x * kHalfLog2e, b.y, b.z, b.w); s.c = make_float2(c.x, c.y); s.id = id;
-            // fast-path eligibility (NaNs answer "generic"): alpha = opacity * G can exceed neither 0.99 nor, with
-            // det >= 1e-5 trace^2 (smallest eigenvalue >= 1e-5 trace: ~100x the fp32 rounding of the three products),
-            // can the computed power be positive
-            const float A = a.z, B = a.w, Cc = b.x, tr = A + Cc;
-            const bool fast = (b.y <= 0.99f) && (A > 0.f) && (Cc > 0.f) && (A * Cc - B * B > 1e-5f * tr * tr) &&
-                              (fabsf(a.x) < 1e7f) && (fabsf(a.y) < 1e7f) && (tr < 1e7f);
-            s.generic = fast ? 0u : 1u;
-            sRec[j] = s;
-            m = strip_mask<NH>(a, b, c.w, tx0, ty0);
-        }
-#pragma unroll
-        for (int w = 0; w < NW; w++) {
-            const uint32_t bits = __brev(__ballot_sync(0xffffffffu, (m >> w) & 1u));
-            if (lane == 0) sMask[w][wid + NW * h] = bits;     // word index = j / 32
-        }
-    }
-}
-
-#define GS_Q(v, q) (((q) & 1) ? (v)[(q) >> 1].y : (v)[(q) >> 1].x)
-
-// The approximate evaluation shared by forward and backward: p = log2(e) * power, g = 2^p, a = opacity * g,
-// d = a + nam (nam = -1/255 for a live pixel: sign-exact alpha >= 1/255 test; -inf for a dead one).  Returns true
-// when one of the alphas sits inside the re-evaluation band around 1/255.
-template <int NH>
-__device__ __forceinline__ bool eval_alpha(const SRec& r, const float dx, const float2* dy, const float2* nam, float2* p,
-                                           float2* g, float2* a, float2* d) {
-    const float hA = (r.a.z * dx) * dx, hB = r.a.w * dx;
-#pragma unroll
-    for (int h = 0; h < NH; h++) {
-        const float2 u = fma2(bc(r.b.x), dy[h], bc(hB));          // C2 dy + B2 dx
-        p[h] = fma2(u, dy[h], bc(hA));                            // (C2 dy + B2 dx) dy + A2 dx dx
-        g[h] = make_float2(ex2_approx(p[h].x), ex2_approx(p[h].y));
-        a[h] = mul2(bc(r.b.y), g[h]);
-        d[h] = add2(a[h], nam[h]);
-    }
-    float m = fminf(fabsf(d[0].x), fabsf(d[0].y));
-    if (NH == 2) m = fminf(m, fminf(fabsf(d[NH - 1].x), fabsf(d[NH - 1].y)));
-    return m < kBand;
-}
-
-// power and alpha (before the 0.99 clamp) of the thread's pixels with the reference's arithmetic (forward.cu:330-343),
-// from the unscaled record
-template <int NH>
-__device__ __forceinline__ void exact_eval(const SRec& r, const float dx, const float2* dy,
-                                           const float4* __restrict__ rec, float* power, float* alpha) {
-    const float4 ra = __ldg(rec + (size_t)GS_REC_V4 * r.id), rb = __ldg(rec + (size_t)GS_REC_V4 * r.id + 1);
-#pragma unroll
-    for (int q = 0; q < 2 * NH; q++) {
-        const float dyq = GS_Q(dy, q);
-        power[q] = -0.5f * (ra.z * dx * dx + rb.x * dyq * dyq) - ra.w * dx * dyq;
-        alpha[q] = r.b.y * expf(power[q]);
-    }
-}
 
 // the thread's pixels as packed pairs: pair h holds image rows pyb + 4h and pyb + 4h + 2
 template <int NH> struct FwdPix {
@@ -260,7 +127,7 @@ k_blend_fwd(const GsView v, const uint32_t* __restrict__ tile_off, const uint32_
     for (int base = 0; base < n; base += kBatch) {
         if (__syncthreads_and(all_dead())) break;
         const int cnt = min(kBatch, n - base);
-        stage_batch<NH>(sRec, sMask, list, rec, beg, cnt, tx0, ty0, [&](int j) { return base + j; });
+        stage_batch<NH, kBatch>(sRec, sMask, list, rec, beg, cnt, tx0, ty0, [&](int j) { return base + j; });
         __syncthreads();
 #pragma unroll 1
         for (int k = 0; k < kWords; k++) {
@@ -357,78 +224,6 @@ __device__ __forceinline__ void warp_reduce9(float* v, const int lane) {
     halving_step<1, 1>(v, lane);
 }
 
-template <int NH> struct BwdPix {
-    float2 T[NH];
-    float2 tb[NH];                    // -T_final * (bg . dL_dpixel)
-    float2 AR[NH];                    // sum_ch accum_rec_ch * dL_dpixel_ch, already advanced past the last contributing splat
-    float2 g0[NH], g1[NH], g2[NH];    // dL_dpixel
-    int last[2 * NH];                 // last contributor (1-based list position)
-};
-
-// What both backward paths sum per (thread, splat), for w = opacity * G * dL_dalpha of the contributing pixels:
-//   vv[0..2] = sum alpha T dL_dpixel_ch          (dL_dcolor)
-//   vv[3..8] = sum w, dx w, sum w dy, dx dx w, dx sum w dy, sum w dy dy
-// backward.cu:563-583 needs G dL_dalpha times {1, dx, dy, dx dx, dx dy, dy dy} and the splat's constants (A, B, C,
-// -0.5 W, -0.5 H, -0.5, 1/opacity), which are applied once per (tile, splat) at the flush.
-//
-// backward.cu:520-528 keeps accum_rec per channel and forms sum_ch (c_ch - accum_rec_ch) * dL_dpixel_ch.  dL_dpixel is
-// constant per pixel, so only the scalar AR = sum_ch accum_rec_ch * dL_dpixel_ch is carried: it obeys the same
-// recurrence (AR' = a cg + (1 - a) AR = AR + a (cg - AR), cg = c . dL_dpixel) and is advanced eagerly.
-
-// generic path of the backward: the reference's test sequence per pixel, exact alpha inside the band
-template <int NH>
-__device__ __forceinline__ bool bwd_generic(BwdPix<NH>& Q, const SRec& r, const float dx, const float2* dy, const float2* p,
-                                            const float2* g, const float2* a, const bool band, const int pos,
-                                            const float4* __restrict__ rec, float* vv) {
-    (void)g;
-    float alpha[2 * NH], power[2 * NH];          // alpha = opacity * G, unclamped
-#pragma unroll
-    for (int q = 0; q < 2 * NH; q++) { alpha[q] = GS_Q(a, q); power[q] = GS_Q(p, q); }
-    if (band || r.generic) exact_eval<NH>(r, dx, dy, rec, power, alpha);
-    bool any = false;
-    float s0 = 0.f, sy = 0.f, syy = 0.f;
-#pragma unroll
-    for (int q = 0; q < 2 * NH; q++) {
-        const float al = fminf(0.99f, alpha[q]);
-        const bool ok = (pos < Q.last[q]) && !(power[q] > 0.0f) && !(al < kAlphaMin);
-        any = any || ok;
-        const float a_ = ok ? al : 0.f;                     // alpha = 0 makes every update below a no-op
-        const float inv = rcp_approx(1.f - a_);
-        float& T = GS_Q(Q.T, q);
-        T = T * inv;
-        const float g0 = GS_Q(Q.g0, q), g1 = GS_Q(Q.g1, q), g2 = GS_Q(Q.g2, q);
-        const float cg = fmaf(r.c.x, g2, fmaf(r.b.w, g1, r.b.z * g0));
-        float& AR = GS_Q(Q.AR, q);
-        const float dcol = cg - AR;
-        AR = fmaf(a_, dcol, AR);
-        const float dch = a_ * T;
-        vv[0] = fmaf(dch, g0, vv[0]); vv[1] = fmaf(dch, g1, vv[1]); vv[2] = fmaf(dch, g2, vv[2]);
-        const float dL_dalpha = fmaf(dcol, T, GS_Q(Q.tb, q) * inv);
-        const float oG = ok ? alpha[q] : 0.f;               // opacity * G; zero keeps an inf of a skipped splat out of the sums
-        const float wq = oG * dL_dalpha;
-        const float dyq = GS_Q(dy, q);
-        s0 += wq;
-        const float t = wq * dyq;
-        sy += t;
-        syy = fmaf(t, dyq, syy);
-    }
-    vv[3] = s0;  vv[4] = dx * s0;  vv[5] = sy;
-    vv[6] = dx * vv[4];  vv[7] = dx * sy;  vv[8] = syy;
-    return any;
-}
-
-// The nine values one (tile, splat) contributes to the splat's accumulator, from the tile sums r[0..8] (see
-// BwdPix): what k_blend_bwd adds into acc and what k_tile_partials stores.  Both kernels run this one expression.
-__device__ __forceinline__ void flush_values(const SRec& sr, const float* r, const float ddelx_dx, const float ddely_dy,
-                                             float4& f0, float4& f1, float& f2) {
-    // r[3..8] = sums of w, w dx, w dy, w dx dx, w dx dy, w dy dy (w = opacity G dL_dalpha) over the tile
-    const float A = sr.a.z * kUnscale, B = sr.a.w * (0.5f * kUnscale), C = sr.b.x * kUnscale;
-    const float kx = r[4], ky = r[5], hf = -0.5f;
-    f0 = make_float4(-(A * kx + B * ky) * ddelx_dx, -(C * ky + B * kx) * ddely_dy, hf * r[6], hf * r[7]);
-    f1 = make_float4(hf * r[8], r[3] * rcp_approx(sr.b.y), r[0], r[1]);
-    f2 = r[2];
-}
-
 // The backward tile pass, shared by both flushes.  PARTS = false (k_blend_bwd): every (tile, splat) leaves the CTA as
 // vector reductions into acc.  PARTS = true (k_tile_partials, the deterministic backward): the nine values of the pair
 // at list position r (tile_off[tile] + pos) are STORED into part_a[2r], part_a[2r+1], part_b[r], and every pair of the
@@ -509,7 +304,7 @@ __device__ __forceinline__ void blend_bwd_tile(const GsView v, const uint32_t* _
         __syncthreads();
         const int cnt = min(kBatch, hi);
         // slot j holds list position hi-1-j: reverse traversal = increasing j
-        stage_batch<NH>(sRec, sMask, list, rec, beg, cnt, tx0, ty0, [&](int j) { return hi - 1 - j; });
+        stage_batch<NH, kBatch>(sRec, sMask, list, rec, beg, cnt, tx0, ty0, [&](int j) { return hi - 1 - j; });
         __syncthreads();
 #pragma unroll 1
         for (int k = 0; k < kWords; k++) {
@@ -639,7 +434,7 @@ int g_gs_blend_variant = 0;           // GS_BLEND_VARIANT=2 / 3 force the 16x8 /
 int g_gs_num_sms = 132;           // H100 SXM; replaced by the device's count when a context is created
 
 // 16x4 strips (4 warps per tile) when 16x8 blocks would leave the SMs with fewer than ~20 resident warps
-static bool use_strips(const GsView& v) {
+bool gs_blend_use_strips(const GsView& v) {
     if (g_gs_blend_variant == 2) return false;
     if (g_gs_blend_variant == 3) return true;
     return (long long)v.gx * v.gy * 2 < (long long)g_gs_num_sms * 20;
@@ -652,33 +447,33 @@ void gs_launch_blend_fwd(const GsView& v, const uint32_t* tile_off, const uint32
     // CTAs per SM the register allocation aims at: 14 (72 registers, 28 warps per SM); 12 (80 registers) measured the same
     // on config 3 (H100 SXM, 400 W limit: 0.127 vs 0.128 ms); GS_BLEND_OCC_FWD=12 keeps the other build for A/B runs
     static const int occ = getenv("GS_BLEND_OCC_FWD") ? atoi(getenv("GS_BLEND_OCC_FWD")) : 14;
-    if (use_strips(v))
+    if (gs_blend_use_strips(v))
         k_blend_fwd<1, 6><<<grid, Geo<1>::NT, 0, s>>>(v, tile_off, list, rec, status, capacity, final_T, n_contrib, out_color, out_depth);
     else if (occ == 12)
         k_blend_fwd<2, 12><<<grid, Geo<2>::NT, 0, s>>>(v, tile_off, list, rec, status, capacity, final_T, n_contrib, out_color, out_depth);
     else
         k_blend_fwd<2, 14><<<grid, Geo<2>::NT, 0, s>>>(v, tile_off, list, rec, status, capacity, final_T, n_contrib, out_color, out_depth);
 }
-void gs_launch_blend_bwd(const GsView& v, const uint32_t* tile_off, const uint32_t* list, const float4* rec,
-                         const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, float4* acc,
-                         const GsDevStatus* status, long long capacity, cudaStream_t s) {
+void gs_launch_blend_bwd_shfl(const GsView& v, const uint32_t* tile_off, const uint32_t* list, const float4* rec,
+                              const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, float4* acc,
+                              const GsDevStatus* status, long long capacity, cudaStream_t s) {
     dim3 grid(v.gx, v.gy);
     // 13 CTAs per SM (72 registers, 4 bytes spilled; shared memory then limits at 13): 0.258 ms against 0.267-0.275 ms
     // for 10 (88 registers) on config 3 (H100 SXM, 400 W limit)
     static const int occ = getenv("GS_BLEND_OCC_BWD") ? atoi(getenv("GS_BLEND_OCC_BWD")) : 13;
-    if (use_strips(v))
+    if (gs_blend_use_strips(v))
         k_blend_bwd<1, 7><<<grid, Geo<1>::NT, 0, s>>>(v, tile_off, list, rec, final_T, n_contrib, dL_dpix, acc, status, capacity);
     else if (occ == 10)
         k_blend_bwd<2, 10><<<grid, Geo<2>::NT, 0, s>>>(v, tile_off, list, rec, final_T, n_contrib, dL_dpix, acc, status, capacity);
     else
         k_blend_bwd<2, 13><<<grid, Geo<2>::NT, 0, s>>>(v, tile_off, list, rec, final_T, n_contrib, dL_dpix, acc, status, capacity);
 }
-void gs_launch_tile_partials(const GsView& v, const uint32_t* tile_off, const uint32_t* list, const float4* rec,
-                             const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, float4* part_a,
-                             float* part_b, const GsDevStatus* status, long long capacity, cudaStream_t s) {
+void gs_launch_tile_partials_shfl(const GsView& v, const uint32_t* tile_off, const uint32_t* list, const float4* rec,
+                                  const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, float4* part_a,
+                                  float* part_b, const GsDevStatus* status, long long capacity, cudaStream_t s) {
     dim3 grid(v.gx, v.gy);
-    // same geometry choice and register targets as gs_launch_blend_bwd
-    if (use_strips(v))
+    // same geometry choice and register targets as gs_launch_blend_bwd_shfl
+    if (gs_blend_use_strips(v))
         k_tile_partials<1, 7><<<grid, Geo<1>::NT, 0, s>>>(v, tile_off, list, rec, final_T, n_contrib, dL_dpix, part_a, part_b,
                                                           status, capacity);
     else
