@@ -7,7 +7,6 @@
 #include <mutex>
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 
 #include "../../include/gsraster.h"
@@ -178,8 +177,6 @@ int gs_context_create(int device, GsContext** out) {
     gs_det_bwd_init();
     gs_grad_write_init();
     gs_preprocess_init();
-    if (const char* e = getenv("GS_BLEND_VARIANT")) g_gs_blend_variant = atoi(e);
-    if (const char* e = getenv("GS_BLEND_BWD")) g_gs_blend_bwd = atoi(e);
     cudaError_t e = cudaHostAlloc((void**)&c->slots, sizeof(GsDevStatus) * (kSlots + kGraphSlots),
                                 cudaHostAllocMapped | cudaHostAllocPortable);
     if (e != cudaSuccess) {
@@ -266,7 +263,6 @@ int gs_forward_preprocess(GsContext* ctx, const GsFrame* f, void* geom_buffer, v
     gs_launch_clear_words(il.tile_cnt, ((size_t)((char*)il.status - (char*)il.tile_cnt) + sizeof(GsDevStatus)) / 4, s);
     GsDevStatus* dev_slot = nullptr;
     GS_CUDA(cudaHostGetDevicePointer((void**)&dev_slot, host_slot, 0));
-    bool scanned = false;
     if (f->P > 0) {
         GsGeomLayout gl = gs_geom_layout(geom_buffer, f->P);
         GS_TIMED(ctx, 0, s, gs_launch_project(v, f->means3D, f->opacities, f->scales, f->rotations, f->cov3D_precomp,
@@ -277,9 +273,7 @@ int gs_forward_preprocess(GsContext* ctx, const GsFrame* f, void* geom_buffer, v
         GS_TIMED(ctx, 8, s, gs_launch_count_tiles(v, ctx->num_sms, radii, gl.rec, gl.vis_list, gl.hitmask, il.tile_cnt, il.status,
                                                   il.tile_off, dev_slot, s));
         if ((rc = debug_sync(f, s, "count_tiles"))) return rc;
-        scanned = gs_scan_folded();
-    }
-    if (!scanned) {
+    } else {                                             // no Gaussians: k_count_tiles does not run, scan the empty histogram
         GS_TIMED(ctx, 1, s, gs_launch_tile_scan(G, il.tile_cnt, il.tile_off, il.status, dev_slot, s));
         if ((rc = debug_sync(f, s, "tile_scan"))) return rc;
     }
@@ -444,7 +438,7 @@ static bool dense_eligible(const GsFrame* f, const GsGrads* grads, const GsGradP
     return grads->peer_world <= 0 && f->shs && f->M == 16 && !f->cov3D_precomp && f->scales && f->rotations &&
            !grads->dL_dcolors && !grads->dL_dcov3D && g.dmeans3D && g.dmeans2D && g.dsh && g.dopacity && g.dscales &&
            g.drots && al16(f->means3D) && al16(f->scales) && al16(g.dmeans3D) && al16(g.dmeans2D) && al16(g.dsh) &&
-           al16(g.dopacity) && al16(g.dscales) && al16(g.drots) && !getenv("GS_NO_DENSE");
+           al16(g.dopacity) && al16(g.dscales) && al16(g.drots);
 }
 
 static int ensure_aux(GsContext* ctx) {
@@ -476,8 +470,7 @@ static int backward_prefill(GsContext* ctx, const GsFrame* f, const void* image_
     int rc = check_frame(f);
     if (rc) return rc;
     ctx->prefilled = nullptr;
-    if (f->P == 0 || !image_buffer || grads->peer_world > 0 || (f->P & 3) || f->cov3D_precomp || !f->scales || !f->rotations ||
-        getenv("GS_NO_PREFILL"))
+    if (f->P == 0 || !image_buffer || grads->peer_world > 0 || (f->P & 3) || f->cov3D_precomp || !f->scales || !f->rotations)
         return GS_OK;
     const GsGradPtrs g = grad_ptrs(f, grads);
     if (!gs_grads_tma_ok(f->shs ? f->M : 0, g)) return GS_OK;

@@ -1,6 +1,6 @@
-// Device pieces shared by the tile-compositing passes (gs_blend.cu: forward and the shuffle-reduction backward;
-// gs_blend_bwd.cu: the slab-reduction backward).  Everything here is per (pixel, splat) arithmetic, staging and the
-// per-(tile, splat) flush; the passes differ only in how they traverse and reduce.  See gs_blend.cu for the design.
+// Device pieces shared by the tile-compositing passes, forward (gs_blend.cu) and backward (gs_blend_bwd.cu): the warp
+// geometries, the staged splat record, FP32 pair arithmetic, staging with the per-strip hit masks, and the alpha
+// evaluation both passes run up to the same skip decision.  See gs_blend.cu for the design.
 #pragma once
 
 #include "gs_common.cuh"
@@ -27,7 +27,6 @@ struct __align__(16) SRec {           // shared-memory copy of a splat record
 };
 
 constexpr float kHalfLog2e = -0.5f * 1.4426950408889634f;     // staged conic scale (see stage_batch)
-constexpr float kUnscale = -2.0f * 0.6931471805599453f;       // back to the conic for the flush of the backward pass
 constexpr float kAlphaMin = 1.0f / 255.0f;
 constexpr float kBand = 1e-7f;
 constexpr float kNegInf = -__builtin_huge_valf();
@@ -142,78 +141,6 @@ __device__ __forceinline__ void exact_eval(const SRec& r, const float dx, const 
         power[q] = -0.5f * (ra.z * dx * dx + rb.x * dyq * dyq) - ra.w * dx * dyq;
         alpha[q] = r.b.y * expf(power[q]);
     }
-}
-
-template <int NH> struct BwdPix {
-    float2 T[NH];
-    float2 tb[NH];                    // -T_final * (bg . dL_dpixel)
-    float2 AR[NH];                    // sum_ch accum_rec_ch * dL_dpixel_ch, already advanced past the last contributing splat
-    float2 g0[NH], g1[NH], g2[NH];    // dL_dpixel
-    int last[2 * NH];                 // last contributor (1-based list position)
-};
-
-// What both backward paths sum per (thread, splat), for w = opacity * G * dL_dalpha of the contributing pixels:
-//   vv[0..2] = sum alpha T dL_dpixel_ch          (dL_dcolor)
-//   vv[3..8] = sum w, dx w, sum w dy, dx dx w, dx sum w dy, sum w dy dy
-// backward.cu:563-583 needs G dL_dalpha times {1, dx, dy, dx dx, dx dy, dy dy} and the splat's constants (A, B, C,
-// -0.5 W, -0.5 H, -0.5, 1/opacity), which are applied once per (tile, splat) at the flush.
-//
-// backward.cu:520-528 keeps accum_rec per channel and forms sum_ch (c_ch - accum_rec_ch) * dL_dpixel_ch.  dL_dpixel is
-// constant per pixel, so only the scalar AR = sum_ch accum_rec_ch * dL_dpixel_ch is carried: it obeys the same
-// recurrence (AR' = a cg + (1 - a) AR = AR + a (cg - AR), cg = c . dL_dpixel) and is advanced eagerly.
-
-// generic path of the backward: the reference's test sequence per pixel, exact alpha inside the band
-template <int NH>
-__device__ __forceinline__ bool bwd_generic(BwdPix<NH>& Q, const SRec& r, const float dx, const float2* dy, const float2* p,
-                                            const float2* g, const float2* a, const bool band, const int pos,
-                                            const float4* __restrict__ rec, float* vv) {
-    (void)g;
-    float alpha[2 * NH], power[2 * NH];          // alpha = opacity * G, unclamped
-#pragma unroll
-    for (int q = 0; q < 2 * NH; q++) { alpha[q] = GS_Q(a, q); power[q] = GS_Q(p, q); }
-    if (band || r.generic) exact_eval<NH>(r, dx, dy, rec, power, alpha);
-    bool any = false;
-    float s0 = 0.f, sy = 0.f, syy = 0.f;
-#pragma unroll
-    for (int q = 0; q < 2 * NH; q++) {
-        const float al = fminf(0.99f, alpha[q]);
-        const bool ok = (pos < Q.last[q]) && !(power[q] > 0.0f) && !(al < kAlphaMin);
-        any = any || ok;
-        const float a_ = ok ? al : 0.f;                     // alpha = 0 makes every update below a no-op
-        const float inv = rcp_approx(1.f - a_);
-        float& T = GS_Q(Q.T, q);
-        T = T * inv;
-        const float g0 = GS_Q(Q.g0, q), g1 = GS_Q(Q.g1, q), g2 = GS_Q(Q.g2, q);
-        const float cg = fmaf(r.c.x, g2, fmaf(r.b.w, g1, r.b.z * g0));
-        float& AR = GS_Q(Q.AR, q);
-        const float dcol = cg - AR;
-        AR = fmaf(a_, dcol, AR);
-        const float dch = a_ * T;
-        vv[0] = fmaf(dch, g0, vv[0]); vv[1] = fmaf(dch, g1, vv[1]); vv[2] = fmaf(dch, g2, vv[2]);
-        const float dL_dalpha = fmaf(dcol, T, GS_Q(Q.tb, q) * inv);
-        const float oG = ok ? alpha[q] : 0.f;               // opacity * G; zero keeps an inf of a skipped splat out of the sums
-        const float wq = oG * dL_dalpha;
-        const float dyq = GS_Q(dy, q);
-        s0 += wq;
-        const float t = wq * dyq;
-        sy += t;
-        syy = fmaf(t, dyq, syy);
-    }
-    vv[3] = s0;  vv[4] = dx * s0;  vv[5] = sy;
-    vv[6] = dx * vv[4];  vv[7] = dx * sy;  vv[8] = syy;
-    return any;
-}
-
-// The nine values one (tile, splat) contributes to the splat's accumulator, from the tile sums r[0..8] (see
-// BwdPix): what k_blend_bwd adds into acc and what k_tile_partials stores.  Both kernels run this one expression.
-__device__ __forceinline__ void flush_values(const SRec& sr, const float* r, const float ddelx_dx, const float ddely_dy,
-                                             float4& f0, float4& f1, float& f2) {
-    // r[3..8] = sums of w, w dx, w dy, w dx dx, w dx dy, w dy dy (w = opacity G dL_dalpha) over the tile
-    const float A = sr.a.z * kUnscale, B = sr.a.w * (0.5f * kUnscale), C = sr.b.x * kUnscale;
-    const float kx = r[4], ky = r[5], hf = -0.5f;
-    f0 = make_float4(-(A * kx + B * ky) * ddelx_dx, -(C * ky + B * kx) * ddely_dy, hf * r[6], hf * r[7]);
-    f1 = make_float4(hf * r[8], r[3] * rcp_approx(sr.b.y), r[0], r[1]);
-    f2 = r[2];
 }
 
 }  // namespace

@@ -1,19 +1,18 @@
-// Backward tile pass with a transposed shared-memory reduction (sm_90a): k_blend_bwd and k_tile_partials.
+// Backward tile pass (sm_90a): k_blend_bwd and k_tile_partials, the reverse traversal of gs_blend.cu's forward.
 //
-// Same traversal and per-pixel arithmetic as the shuffle-butterfly pass of gs_blend.cu (shared device functions of
-// gs_blend.cuh, fast path operation for operation); only the path from a lane's nine per-splat values vv[0..8] to the
-// per-(tile, splat) sums differs.  The butterfly spent ~72 warp instructions per (warp, splat) on 12 SHFL, their
-// selects and adds, for 9 useful additions.  Here:
+// Staging, the alpha evaluation and the skip decision are the forward's (gs_blend.cuh).  Per hit splat every lane
+// computes nine values vv[0..8] for its pixels (BwdPix), and the per-(tile, splat) sums are formed as follows:
 //  * each warp buffers the lanes' values of kGroup = 3 hit splats in its own slab, [splat][value][lane] (27 rows of
 //    32 lanes, rows padded to 36 words): 9 plain STS per splat, conflict-free;
 //  * when the slab is full (or the batch ends), lane i < 27 sums row i: 8 LDS.128 (8 consecutive lanes read 8
-//    distinct 4-bank groups thanks to the padding) and 31 FADD, in the butterfly's tree order -- pairs (l, l^16)
-//    first, then bits 3, 2, 1, 0 -- so every sum is bit-identical to gs_blend.cu's;
-//  * the sum goes to the warp's per-splat slot in shared memory, and the CTA sums the warps and flushes exactly as
-//    gs_blend.cu does (flush_values, then red.global.add.v4.f32 or the stores of the deterministic partials).
+//    distinct 4-bank groups thanks to the padding) and 31 FADD in a fixed tree order -- pairs (l, l^16) first, then
+//    the partials 8, 4, 2, 1 apart (slab_row_sum);
+//  * the sum goes to the warp's per-splat slot in shared memory, and the CTA sums the warps and flushes the sums
+//    (flush_values, then red.global.add.v4.f32 or the stores of the deterministic partials).
+// That tree order is the deterministic backward's contract: k_tile_partials stores its sums, and gs_det_bwd.cu adds
+// them in a fixed order, so changing the tree changes the deterministic gradients' bits.
 // The slab costs 3.9 KB per warp; the batch is 64 splats (config 3 has ~49 pairs per tile after exact culling), which
-// keeps shared memory per CTA at gs_blend.cu's 15 KB (NH = 2).
-#include <cstdlib>
+// keeps shared memory per CTA at 15 KB (NH = 2).
 
 #include "gs_blend.cuh"
 
@@ -24,6 +23,80 @@ constexpr int kWords = kBatch / 32;
 constexpr int kGroup = 3;             // hit splats per slab: 27 (splat, value) rows, one per lane
 constexpr int kRows = 9 * kGroup;
 constexpr int kStride = 36;           // slab row: 32 lanes + 4 words of padding (16-byte aligned rows)
+
+constexpr float kUnscale = -2.0f * 0.6931471805599453f;   // undoes stage_batch's conic scaling for the flush
+
+template <int NH> struct BwdPix {
+    float2 T[NH];
+    float2 tb[NH];                    // -T_final * (bg . dL_dpixel)
+    float2 AR[NH];                    // sum_ch accum_rec_ch * dL_dpixel_ch, already advanced past the last contributing splat
+    float2 g0[NH], g1[NH], g2[NH];    // dL_dpixel
+    int last[2 * NH];                 // last contributor (1-based list position)
+};
+
+// What both backward paths sum per (thread, splat), for w = opacity * G * dL_dalpha of the contributing pixels:
+//   vv[0..2] = sum alpha T dL_dpixel_ch          (dL_dcolor)
+//   vv[3..8] = sum w, dx w, sum w dy, dx dx w, dx sum w dy, sum w dy dy
+// backward.cu:563-583 needs G dL_dalpha times {1, dx, dy, dx dx, dx dy, dy dy} and the splat's constants (A, B, C,
+// -0.5 W, -0.5 H, -0.5, 1/opacity), which are applied once per (tile, splat) at the flush.
+//
+// backward.cu:520-528 keeps accum_rec per channel and forms sum_ch (c_ch - accum_rec_ch) * dL_dpixel_ch.  dL_dpixel is
+// constant per pixel, so only the scalar AR = sum_ch accum_rec_ch * dL_dpixel_ch is carried: it obeys the same
+// recurrence (AR' = a cg + (1 - a) AR = AR + a (cg - AR), cg = c . dL_dpixel) and is advanced eagerly.
+
+// generic path of the backward: the reference's test sequence per pixel, exact alpha inside the band
+template <int NH>
+__device__ __forceinline__ bool bwd_generic(BwdPix<NH>& Q, const SRec& r, const float dx, const float2* dy, const float2* p,
+                                            const float2* g, const float2* a, const bool band, const int pos,
+                                            const float4* __restrict__ rec, float* vv) {
+    (void)g;
+    float alpha[2 * NH], power[2 * NH];          // alpha = opacity * G, unclamped
+#pragma unroll
+    for (int q = 0; q < 2 * NH; q++) { alpha[q] = GS_Q(a, q); power[q] = GS_Q(p, q); }
+    if (band || r.generic) exact_eval<NH>(r, dx, dy, rec, power, alpha);
+    bool any = false;
+    float s0 = 0.f, sy = 0.f, syy = 0.f;
+#pragma unroll
+    for (int q = 0; q < 2 * NH; q++) {
+        const float al = fminf(0.99f, alpha[q]);
+        const bool ok = (pos < Q.last[q]) && !(power[q] > 0.0f) && !(al < kAlphaMin);
+        any = any || ok;
+        const float a_ = ok ? al : 0.f;                     // alpha = 0 makes every update below a no-op
+        const float inv = rcp_approx(1.f - a_);
+        float& T = GS_Q(Q.T, q);
+        T = T * inv;
+        const float g0 = GS_Q(Q.g0, q), g1 = GS_Q(Q.g1, q), g2 = GS_Q(Q.g2, q);
+        const float cg = fmaf(r.c.x, g2, fmaf(r.b.w, g1, r.b.z * g0));
+        float& AR = GS_Q(Q.AR, q);
+        const float dcol = cg - AR;
+        AR = fmaf(a_, dcol, AR);
+        const float dch = a_ * T;
+        vv[0] = fmaf(dch, g0, vv[0]); vv[1] = fmaf(dch, g1, vv[1]); vv[2] = fmaf(dch, g2, vv[2]);
+        const float dL_dalpha = fmaf(dcol, T, GS_Q(Q.tb, q) * inv);
+        const float oG = ok ? alpha[q] : 0.f;               // opacity * G; zero keeps an inf of a skipped splat out of the sums
+        const float wq = oG * dL_dalpha;
+        const float dyq = GS_Q(dy, q);
+        s0 += wq;
+        const float t = wq * dyq;
+        sy += t;
+        syy = fmaf(t, dyq, syy);
+    }
+    vv[3] = s0;  vv[4] = dx * s0;  vv[5] = sy;
+    vv[6] = dx * vv[4];  vv[7] = dx * sy;  vv[8] = syy;
+    return any;
+}
+
+// The nine values one (tile, splat) contributes to the splat's accumulator, from the tile sums r[0..8] (see
+// BwdPix): what k_blend_bwd adds into acc and what k_tile_partials stores.  Both kernels run this one expression.
+__device__ __forceinline__ void flush_values(const SRec& sr, const float* r, const float ddelx_dx, const float ddely_dy,
+                                             float4& f0, float4& f1, float& f2) {
+    // r[3..8] = sums of w, w dx, w dy, w dx dx, w dx dy, w dy dy (w = opacity G dL_dalpha) over the tile
+    const float A = sr.a.z * kUnscale, B = sr.a.w * (0.5f * kUnscale), C = sr.b.x * kUnscale;
+    const float kx = r[4], ky = r[5], hf = -0.5f;
+    f0 = make_float4(-(A * kx + B * ky) * ddelx_dx, -(C * ky + B * kx) * ddely_dy, hf * r[6], hf * r[7]);
+    f1 = make_float4(hf * r[8], r[3] * rcp_approx(sr.b.y), r[0], r[1]);
+    f2 = r[2];
+}
 
 // The slab and the staged records are read and written through 32-bit shared-window addresses (ld/st.shared): the
 // slab's stores and loads stay in the order the __syncwarp()s give them, and the record's fields are plain loads the
@@ -59,9 +132,8 @@ __device__ __forceinline__ SRec load_srec(const uint32_t addr) {
     return r;
 }
 
-// Lane i < 9 * n sums slab row i over the 32 lanes in the order of gs_blend.cu's warp_reduce9 butterfly: element l is
-// first added to element l + 16, then the partials to the one 8, 4, 2, 1 further.  Float addition is commutative, so
-// this tree gives the butterfly's bits.
+// Lane i < 9 * n sums slab row i over the 32 lanes: element l is first added to element l + 16, then the partials to the
+// one 8, 4, 2, 1 further.  The deterministic backward's gradients depend on this order bit for bit.
 __device__ __forceinline__ float slab_row_sum(const uint32_t row) {
     float4 s1[4];
 #pragma unroll
@@ -77,8 +149,10 @@ __device__ __forceinline__ float slab_row_sum(const uint32_t row) {
     return (s3.x + s3.z) + (s3.y + s3.w);
 }
 
-// gs_blend.cu's blend_bwd_tile with the slab reduction; PARTS as there (k_tile_partials stores the nine values of every
-// pair, zeros for pairs no pixel reached).
+// The backward tile pass, shared by both flushes.  PARTS = false (k_blend_bwd): every (tile, splat) leaves the CTA as
+// vector reductions into acc.  PARTS = true (k_tile_partials, the deterministic backward): the nine values of the pair
+// at list position r (tile_off[tile] + pos) are STORED into part_a[2r], part_a[2r+1], part_b[r], and every pair of the
+// tile that no pixel reached gets zeros, so all num_pairs entries are defined after the pass.
 template <int NH, bool PARTS>
 __device__ __forceinline__ void blend_bwd_tile_slab(const GsView v, const uint32_t* __restrict__ tile_off,
                                                     const uint32_t* __restrict__ list, const float4* __restrict__ rec,
@@ -303,16 +377,10 @@ k_tile_partials(const GsView v, const uint32_t* __restrict__ tile_off, const uin
 
 }  // namespace
 
-int g_gs_blend_bwd = 1;               // GS_BLEND_BWD=0: gs_blend.cu's shuffle-butterfly backward (A/B measurements)
-
-// Register targets as gs_blend.cu's: 13 CTAs per SM for 16x8 blocks, 7 for 16x4 strips
+// Register targets: 13 CTAs per SM for 16x8 blocks, 7 for 16x4 strips
 void gs_launch_blend_bwd(const GsView& v, const uint32_t* tile_off, const uint32_t* list, const float4* rec,
                          const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, float4* acc,
                          const GsDevStatus* status, long long capacity, cudaStream_t s) {
-    if (!g_gs_blend_bwd) {
-        gs_launch_blend_bwd_shfl(v, tile_off, list, rec, final_T, n_contrib, dL_dpix, acc, status, capacity, s);
-        return;
-    }
     dim3 grid(v.gx, v.gy);
     if (gs_blend_use_strips(v))
         k_blend_bwd<1, 7><<<grid, Geo<1>::NT, 0, s>>>(v, tile_off, list, rec, final_T, n_contrib, dL_dpix, acc, status, capacity);
@@ -322,10 +390,6 @@ void gs_launch_blend_bwd(const GsView& v, const uint32_t* tile_off, const uint32
 void gs_launch_tile_partials(const GsView& v, const uint32_t* tile_off, const uint32_t* list, const float4* rec,
                              const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, float4* part_a,
                              float* part_b, const GsDevStatus* status, long long capacity, cudaStream_t s) {
-    if (!g_gs_blend_bwd) {
-        gs_launch_tile_partials_shfl(v, tile_off, list, rec, final_T, n_contrib, dL_dpix, part_a, part_b, status, capacity, s);
-        return;
-    }
     dim3 grid(v.gx, v.gy);
     if (gs_blend_use_strips(v))
         k_tile_partials<1, 7><<<grid, Geo<1>::NT, 0, s>>>(v, tile_off, list, rec, final_T, n_contrib, dL_dpix, part_a, part_b,

@@ -329,7 +329,6 @@ struct GsGradPtrs {
 void gs_launch_project(const GsView& v, const float* means3D, const float* opacities, const float* scales,
                        const float* rotations, const float* cov3D_precomp, int* radii, float4* rec,
                        uint32_t* vis_list, GsDevStatus* status, bool dense_hint, cudaStream_t s);
-bool gs_scan_folded();   // true: the last CTA of k_count_tiles scans the tile histogram, no k_tile_scan launch follows
 void gs_launch_count_tiles(const GsView& v, int num_sms, const int* radii, const float4* rec, const uint32_t* vis_list,
                            uint32_t* hitmask, uint32_t* tile_cnt, GsDevStatus* status, uint32_t* tile_off,
                            GsDevStatus* host_slot, cudaStream_t s);
@@ -354,19 +353,10 @@ void gs_launch_blend_bwd(const GsView& v, const uint32_t* tile_off, const uint32
 void gs_launch_tile_partials(const GsView& v, const uint32_t* tile_off, const uint32_t* list, const float4* rec,
                              const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, float4* part_a,
                              float* part_b, const GsDevStatus* status, long long capacity, cudaStream_t s);
-// the shuffle-butterfly backward of gs_blend.cu, selected by GS_BLEND_BWD=0 (g_gs_blend_bwd = 0) for A/B runs
-void gs_launch_blend_bwd_shfl(const GsView& v, const uint32_t* tile_off, const uint32_t* list, const float4* rec,
-                              const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, float4* acc,
-                              const GsDevStatus* status, long long capacity, cudaStream_t s);
-void gs_launch_tile_partials_shfl(const GsView& v, const uint32_t* tile_off, const uint32_t* list, const float4* rec,
-                                  const float* final_T, const uint32_t* n_contrib, const float* dL_dpix, float4* part_a,
-                                  float* part_b, const GsDevStatus* status, long long capacity, cudaStream_t s);
 bool gs_blend_use_strips(const GsView& v);
 void gs_det_bwd_init();
 void gs_launch_det_reduce(const GsDetLayout& d, int num_sms, const uint32_t* list, const uint32_t* vis_list, float4* acc,
                           const GsDevStatus* status, long long capacity, cudaStream_t s);
-extern int g_gs_blend_variant;
-extern int g_gs_blend_bwd;
 extern int g_gs_num_sms;
 void gs_launch_grad_vis(const GsView& v, int num_sms, const float* means3D, const float* shs, const float* scales,
                         const float* rotations, const float* cov3D_precomp, const float4* rec, float4* acc,

@@ -11,7 +11,6 @@
 //                 dense [P,*] intermediates (dL_dconic, dL_dcov3D, dL_dcolors never exist as dense tensors unless
 //                 the caller asks for them).  HBM-bound: ~248 B written + 4 B read per Gaussian; every store is a
 //                 fully coalesced 128-bit (dL_dsh, rotations) or 32-bit row-contiguous store.
-#include <cstdlib>
 
 #include "gs_common.cuh"
 
@@ -932,8 +931,7 @@ void gs_launch_grad_vis(const GsView& v, int num_sms, const float* means3D, cons
 bool gs_grads_tma_ok(int M, const GsGradPtrs& g) {
     auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
     return M == 16 && g.dsh && g.dmeans3D && g.dmeans2D && g.dscales && g.dopacity && g.drots && !g.dcolors && !g.dcov3D &&
-           al16(g.dsh) && al16(g.dmeans3D) && al16(g.dmeans2D) && al16(g.dscales) && al16(g.dopacity) && al16(g.drots) &&
-           !getenv("GS_NO_TMA");
+           al16(g.dsh) && al16(g.dmeans3D) && al16(g.dmeans2D) && al16(g.dscales) && al16(g.dopacity) && al16(g.drots);
 }
 void gs_launch_fill_zero(int P, int num_sms, const GsGradPtrs& g, const GsDevStatus* status, bool dense_elsewhere,
                          cudaStream_t s) {
@@ -944,8 +942,7 @@ void gs_launch_fill_zero(int P, int num_sms, const GsGradPtrs& g, const GsDevSta
     r.p[3] = (char*)g.dscales;  r.bytes[3] = (long long)P * 12;
     r.p[4] = (char*)g.dopacity; r.bytes[4] = (long long)P * 4;
     r.p[5] = (char*)g.drots;    r.bytes[5] = (long long)P * 16;
-    static const int ctas = getenv("GS_FILL_CTAS") ? atoi(getenv("GS_FILL_CTAS")) : 0;   // tuning knob (experiments)
-    k_fill_zero<<<ctas > 0 ? ctas : num_sms * 4, 32, 0, s>>>(r, status, P, dense_elsewhere);
+    k_fill_zero<<<num_sms * 4, 32, 0, s>>>(r, status, P, dense_elsewhere);
 }
 // the dense-regime twin of (k_grad_vis, k_grad_write): returns at once on the device unless most Gaussians are visible
 void gs_launch_grad_dense(const GsView& v, int num_sms, const float* means3D, const float* shs, const float* scales,

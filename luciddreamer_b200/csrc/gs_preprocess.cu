@@ -17,7 +17,6 @@
 // Histogram and emission spread the (Gaussian, tile) candidates of a CTA's 256 Gaussians evenly over its threads
 // (block scan of the rect areas + binary search), so a splat covering thousands of tiles costs the same per thread
 // as one covering four.
-#include <cstdlib>
 
 #include "gs_common.cuh"
 
@@ -189,7 +188,7 @@ __device__ __forceinline__ void append_visible(const Projected& o, const int i, 
     }
 }
 
-// One thread per Gaussian, exact path for all of them (the first version of the pass; GS_PROJECT_V1=1 selects it).
+// One thread per Gaussian, exact path for all of them (the first version of the pass; dense frames run it).
 __global__ void __launch_bounds__(kThreads)
 k_project_v1(const GsView v, const float* __restrict__ means3D, const float* __restrict__ opacities,
              const float* __restrict__ scales, const float* __restrict__ rotations, const float* __restrict__ cov3D_precomp,
@@ -451,7 +450,7 @@ __device__ __forceinline__ void cta_tile_scan(const int G, uint32_t* __restrict_
     }
 }
 
-// the scan as a kernel of its own: empty models (no k_count_tiles launch) and GS_SCAN_KERNEL=1
+// the scan as a kernel of its own, for empty models (no k_count_tiles launch)
 constexpr int kScanT = 1024, kScanK = 8;
 __global__ void __launch_bounds__(kScanT)
 k_tile_scan(int G, uint32_t* __restrict__ tile_cnt, uint32_t* __restrict__ tile_off, GsDevStatus* __restrict__ status,
@@ -704,14 +703,9 @@ void gs_launch_project(const GsView& v, const float* means3D, const float* opaci
     const int grid = (v.P + kThreads - 1) / kThreads;
     // most of the model was inside the previous view of this context: the screen pre-test would reject next to nothing
     // -- skip it (same results either way)
-    static const bool v1 = getenv("GS_PROJECT_V1") != nullptr;
     const int pgrid = grid < g_gs_num_sms * 4 ? grid : g_gs_num_sms * 4;      // persistent: 4 CTAs of <= 64 registers per SM
-    if (v1 || dense_hint) k_project_v1<<<grid, kThreads, 0, s>>>(v, means3D, opacities, scales, rotations, cov3D_precomp, radii, rec, vis_list, status);
+    if (dense_hint) k_project_v1<<<grid, kThreads, 0, s>>>(v, means3D, opacities, scales, rotations, cov3D_precomp, radii, rec, vis_list, status);
     else k_project<<<pgrid, kThreads, 0, s>>>(v, means3D, opacities, scales, rotations, cov3D_precomp, radii, rec, vis_list, status);
-}
-bool gs_scan_folded() {
-    static const bool separate = getenv("GS_SCAN_KERNEL") != nullptr;
-    return !separate;
 }
 void gs_launch_count_tiles(const GsView& v, int num_sms, const int* radii, const float4* rec, const uint32_t* vis_list,
                            uint32_t* hitmask, uint32_t* tile_cnt, GsDevStatus* status, uint32_t* tile_off,
@@ -719,7 +713,7 @@ void gs_launch_count_tiles(const GsView& v, int num_sms, const int* radii, const
     const int need = (v.P + kChunkMin - 1) / kChunkMin;
     const int grid = need < num_sms * 8 ? need : num_sms * 8;
     k_count_tiles<<<grid, kThreads, 0, s>>>(v, radii, rec, vis_list, hitmask, tile_cnt, status, tile_off, host_slot,
-                                            gs_scan_folded());
+                                            true);
 }
 void gs_launch_tile_scan(int G, uint32_t* tile_cnt, uint32_t* tile_off, GsDevStatus* status, GsDevStatus* host_slot,
                          cudaStream_t s) {
@@ -737,7 +731,7 @@ void gs_launch_shade_emit(const GsView& v, int num_sms, const float* means3D, co
     // TMA staging of the SH rows: 16 stored coefficients (192-byte rows, 16-byte aligned like the base pointer).  The
     // kernel uses it only when most Gaussians are visible; `dense_hint` (the previous frame on this context) decides
     // whether the launch reserves the 53 KB staging buffer at all -- either way the result is the same.
-    const bool use_tma = dense_hint && shs && !colors_precomp && v.M == 16 && !getenv("GS_NO_TMA");
+    const bool use_tma = dense_hint && shs && !colors_precomp && v.M == 16;
     const size_t smem = use_tma ? (size_t)kChunkMax * kShRow * sizeof(float) : 0;
     const int per_sm = use_tma ? 4 : 8;                  // 53 KB of shared memory per CTA with the staging buffer
     const int grid = need < num_sms * per_sm ? need : num_sms * per_sm;

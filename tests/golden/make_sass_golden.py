@@ -1,6 +1,5 @@
-"""Fingerprints of the machine code of every kernel object that existed before the training-step kernels
-(tests/test_train_cpu.py checks that they stay unchanged).  Run on a build of the commit that introduced gs_train.cu
-with that file's changes reverted, or of its parent:
+"""Fingerprints of the machine code of every kernel of every object (tests/test_train_cpu.py checks that the kernels
+stay unchanged).  Run on a build of the commit whose kernels the golden should pin:
 
     make -C luciddreamer_b200/csrc && python tests/golden/make_sass_golden.py luciddreamer_b200/csrc
 """
@@ -15,19 +14,26 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
-def fingerprint(obj: str) -> str:
-    """sha256 of the SASS listing: function names (the per-path anonymous-namespace tag replaced) and instructions."""
+def kernel_fingerprints(obj: str) -> dict:
+    """{function name: sha256 of its SASS listing}.  The listing is the function name line and the instructions, with
+    the encodings dropped and the anonymous-namespace tags replaced (in the name too): nvcc derives one from the
+    source path and one from the file's contents, so neither says anything about the kernel's machine code."""
     out = subprocess.run(["cuobjdump", "-sass", obj], capture_output=True, text=True, check=True).stdout
-    keep = []
+    per, fn = {}, None
     for line in out.splitlines():
         if "Function :" in line or re.search(r"/\*[0-9a-f]{4}\*/", line):
             line = re.sub(r"_GLOBAL__N__[0-9a-f]{8}_", "_GLOBAL__N__X_", line)
-            keep.append(re.sub(r"/\* 0x[0-9a-f]+ \*/", "", line).strip())
-    return hashlib.sha256("\n".join(keep).encode()).hexdigest()
+            line = re.sub(r"(_GLOBAL__N__X_\d+_\w+?_cu)_[0-9a-f]{8}", r"\1_X", line)
+            line = re.sub(r"/\* 0x[0-9a-f]+ \*/", "", line).strip()
+            if "Function :" in line:
+                fn = line.split("Function :", 1)[1].strip()
+                per[fn] = []
+            per[fn].append(line)
+    return {fn: hashlib.sha256("\n".join(lines).encode()).hexdigest() for fn, lines in per.items()}
 
 
 if __name__ == "__main__":
     objs = sorted(glob.glob(os.path.join(sys.argv[1], "*.o")))
-    gold = {os.path.basename(o): fingerprint(o) for o in objs if not o.endswith("gs_train.o")}
-    json.dump(gold, open(os.path.join(HERE, "sass_before_train.json"), "w"), indent=1, sort_keys=True)
-    print(f"{len(gold)} objects")
+    gold = {os.path.basename(o): kernel_fingerprints(o) for o in objs}
+    json.dump(gold, open(os.path.join(HERE, "sass_kernels.json"), "w"), indent=1, sort_keys=True)
+    print(f"{len(gold)} objects, {sum(len(k) for k in gold.values())} kernels")

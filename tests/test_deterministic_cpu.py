@@ -73,8 +73,8 @@ def _sass(obj):
     return per
 
 
-def test_deterministic_kernels_issue_no_float_reductions():
-    per = {**_sass("gs_blend.o"), **_sass("gs_det_bwd.o")}
+def test_running_deterministic_kernels_issue_no_float_reductions():
+    per = {**_sass("gs_blend_bwd.o"), **_sass("gs_det_bwd.o")}
     new = {k: v for k, v in per.items() if "k_tile_partials" in k or "k_det_" in k}
     assert len([k for k in new if "k_tile_partials" in k]) == 2          # both warp geometries
     for name in ("k_det_count", "k_det_scan_reduce", "k_det_scan_down", "k_det_place", "k_det_sort_warp",

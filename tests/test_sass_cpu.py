@@ -41,15 +41,14 @@ def _kernels(per, key):
     return hit
 
 
-def test_blend_kernels_issue_vector_reductions():
-    per = _sass("gs_blend.o")
-    for name in ("k_blend_fwd", "k_blend_bwd"):
-        for fn, c in _kernels(per, name).items():
+def test_running_blend_kernels_issue_vector_reductions():
+    fwd, bwd = _kernels(_sass("gs_blend.o"), "k_blend_fwd"), _kernels(_sass("gs_blend_bwd.o"), "k_blend_bwd")
+    for kernels in (fwd, bwd):
+        for fn, c in kernels.items():
             assert c["HMMA"] == 0 and c["HGMMA"] == 0                     # no tensor cores on this path
             # double precision: only the two prologue products 0.5 * W, 0.5 * H of the backward (backward.cu:473-474 writes
             # them with a double literal; once per kernel, exact in either precision)
             assert c["DFMA"] == 0 and c["DADD"] == 0 and c["DMUL"] <= 2, (fn, c["DFMA"], c["DADD"], c["DMUL"])
-    bwd = _kernels(per, "k_blend_bwd")
     assert all(any(op.startswith("REDG.E.ADD.F32x4") for op in c) for c in bwd.values()), \
         "the backward tile pass must leave the CTA through 128-bit vector reductions (red.global.add.v4.f32)"
 
