@@ -43,11 +43,9 @@ int check_frame(const GsFrame* f) {
     // RAST/depth_diff_gaussian_rasterization_min/__init__.py:192-196
     if ((f->shs == nullptr) == (f->colors_precomp == nullptr))
         return fail(GS_EINVAL, "Please provide excatly one of either SHs or precomputed colors!");
-    const bool has_sr = f->scales != nullptr && f->rotations != nullptr;
     if (((f->scales == nullptr || f->rotations == nullptr) && f->cov3D_precomp == nullptr) ||
         ((f->scales != nullptr || f->rotations != nullptr) && f->cov3D_precomp != nullptr))
         return fail(GS_EINVAL, "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
-    (void)has_sr;
     // k_project / k_grad_vis / sh_to_rgb read rotations and SH rows with 128-bit loads
     if ((reinterpret_cast<uintptr_t>(f->rotations) & 15) || (reinterpret_cast<uintptr_t>(f->shs) & 15))
         return fail(GS_EINVAL, "rotations and shs must be 16-byte aligned (see gsraster.h)");
@@ -113,8 +111,6 @@ struct GsContext {
     cudaStream_t aux;              // side stream of gs_backward's zero-fill (beside the tile pass) and peer barrier
     cudaEvent_t aux_fork, aux_join;
     bool aux_ready;
-    const void* prefilled;         // dL_dsh pointer of the outputs the most recent prefill was issued for
-    bool peer_barrier_pending;     // the "every bucket is cleared" barrier of this step runs on `aux`
     cudaStream_t vstreams[kMaxViewStreams];   // internal streams of gs_forward_views (created on first use)
     cudaEvent_t vfork, vjoin[kMaxViewStreams];
     bool vstreams_ready;
@@ -165,8 +161,6 @@ int gs_context_create(int device, GsContext** out) {
     c->profile = 0;
     c->vstreams_ready = false;
     c->aux_ready = false;
-    c->prefilled = nullptr;
-    c->peer_barrier_pending = false;
     for (int i = 0; i < kSlots; i++) c->slot_gen[i] = 0;
     for (int i = 0; i < kNumKernels; i++) c->pev_used[i] = false;
     for (int i = 0; i < 2 * kNumKernels; i++) cudaEventCreate(&c->pev[i]);
@@ -431,16 +425,6 @@ static GsGradPtrs grad_ptrs(const GsFrame* f, const GsGrads* grads) {
     return g;
 }
 
-// the dense-regime kernel (k_grad_dense) covers the reference's own input mode: SH degree <= 3 stored as 16 coefficients,
-// scales + rotations, all six gradients wanted; its bulk copies need 16-byte aligned bases (gsraster.h)
-static bool dense_eligible(const GsFrame* f, const GsGrads* grads, const GsGradPtrs& g) {
-    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
-    return grads->peer_world <= 0 && f->shs && f->M == 16 && !f->cov3D_precomp && f->scales && f->rotations &&
-           !grads->dL_dcolors && !grads->dL_dcov3D && g.dmeans3D && g.dmeans2D && g.dsh && g.dopacity && g.dscales &&
-           g.drots && al16(f->means3D) && al16(f->scales) && al16(g.dmeans3D) && al16(g.dmeans2D) && al16(g.dsh) &&
-           al16(g.dopacity) && al16(g.dscales) && al16(g.drots);
-}
-
 static int ensure_aux(GsContext* ctx) {
     if (ctx->aux_ready) return GS_OK;
     int prev = 0;
@@ -459,113 +443,112 @@ static int ensure_aux(GsContext* ctx) {
     return GS_OK;
 }
 
-// First stage of gs_backward, before the tile pass: zero-fills the dense gradient outputs on a side stream of the context,
-// BESIDE the tile pass (which is issue bound and leaves the memory system idle).  backward_gradients then waits for the
-// fill and lets the per-Gaussian kernel write the visible rows straight into the outputs -- the streaming writer of the
-// sparse regime disappears from the critical path.  Returns GS_OK without doing anything when the outputs do not qualify
-// (all six of dL_dmeans3D / dL_dmeans2D / dL_dsh (M = 16) / dL_dopacity / dL_dscales / dL_drotations wanted, bases
-// 16-byte aligned, P a multiple of 4, no peer reduce): backward_gradients falls back to its own writer.
-static int backward_prefill(GsContext* ctx, const GsFrame* f, const void* image_buffer, const GsGrads* grads, gs_stream_t stream) {
-    if (!ctx || !grads) return fail(GS_EINVAL, "ctx / grads is NULL");
-    int rc = check_frame(f);
-    if (rc) return rc;
-    ctx->prefilled = nullptr;
-    if (f->P == 0 || !image_buffer || grads->peer_world > 0 || (f->P & 3) || f->cov3D_precomp || !f->scales || !f->rotations)
-        return GS_OK;
-    const GsGradPtrs g = grad_ptrs(f, grads);
-    if (!gs_grads_tma_ok(f->shs ? f->M : 0, g)) return GS_OK;
-    cudaStream_t s = (cudaStream_t)stream;
-    if ((rc = ensure_aux(ctx))) return rc;
-    GsImageLayout il = gs_image_layout(const_cast<void*>(image_buffer), f->W, f->H);
-    GS_CUDA(cudaEventRecord(ctx->aux_fork, s));            // the outputs were allocated in `stream` order before this call
-    GS_CUDA(cudaStreamWaitEvent(ctx->aux, ctx->aux_fork, 0));
-    // in the dense regime k_grad_dense writes every row itself: the fill exits on the device (only if that kernel will run)
-    GS_TIMED(ctx, 11, ctx->aux, gs_launch_fill_zero(f->P, ctx->num_sms, g, il.status, dense_eligible(f, grads, g), ctx->aux));
-    GS_CUDA(cudaEventRecord(ctx->aux_join, ctx->aux));
-    ctx->prefilled = grads->dL_dsh;
-    return GS_OK;
+// Which kernels write the per-Gaussian gradients of one backward call, decided once from its inputs.
+enum class GradWriter { none, tma, generic };
+struct GradPlan {
+    bool fill;          // k_fill_zero zeroes the outputs on ctx->aux beside the tile pass; k_grad_vis scatters final rows
+    bool dense_ok;      // k_grad_dense covers the input mode: in its regime (decided on the device) the others exit
+    bool dense;         // ... and is launched: the scratch bound does not prove the sparse regime
+    GradWriter writer;  // the writer after k_grad_vis
+    bool peer;          // rows are reduced into every rank's bucket (k_grad_reduce_peers); only dL_dmeans2D is local
+    bool peer_begin;    // the peer route's "every bucket is cleared" barrier waits on ctx->aux beside the tile pass
+};
+
+// `nvis_bound`: compact rows the gradient scratch holds.  The TMA paths (k_fill_zero + scatter, k_grad_write_tma) need
+// the six outputs of the reference's own input mode (16 stored SH coefficients) and nothing else, 16-byte aligned;
+// k_grad_dense also needs scales + rotations and 16-byte aligned means / scales for its bulk copies (gsraster.h); the
+// fill also needs P a multiple of 4 and a context for its side stream.
+static GradPlan grad_plan(const GsContext* ctx, const GsFrame* f, const GsGrads* grads, const GsGradPtrs& g,
+                          long long nvis_bound) {
+    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+    const bool tma_ok = f->shs && f->M == 16 && g.dsh && g.dmeans3D && g.dmeans2D && g.dscales && g.dopacity && g.drots &&
+                        !g.dcolors && !g.dcov3D && al16(g.dsh) && al16(g.dmeans3D) && al16(g.dmeans2D) &&
+                        al16(g.dscales) && al16(g.dopacity) && al16(g.drots);
+    const bool sr = !f->cov3D_precomp && f->scales && f->rotations;
+    GradPlan p;
+    p.peer = grads->peer_world > 0;
+    p.peer_begin = ctx && p.peer && grads->peer_signals && grads->peer_epoch_begin;
+    p.fill = ctx && f->P > 0 && !p.peer && !(f->P & 3) && sr && tma_ok;
+    p.dense_ok = !p.peer && tma_ok && sr && al16(f->means3D) && al16(f->scales);
+    p.dense = p.dense_ok && 2 * nvis_bound > (long long)f->P;
+    p.writer = (p.peer || p.fill) ? GradWriter::none : tma_ok ? GradWriter::tma : GradWriter::generic;
+    return p;
 }
 
-// Backward, tile pass: reverse tile traversal into the per-Gaussian accumulators.
-static int backward_blend(GsContext* ctx, const GsFrame* f, const void* geom_buffer, const void* binning_buffer,
-                      int64_t pair_capacity, const void* image_buffer, const float* dL_dout_color,
-                      gs_stream_t stream) {
+// The backward shared by gs_backward and gs_backward_deterministic once their own arguments are checked.  Tile pass:
+// k_blend_bwd, or (`det` non-NULL) k_tile_partials + the fixed-order reduce.  Beside it on the context's side stream:
+// the zero-fill of the outputs or the peer route's begin barrier.  Then the per-Gaussian writers of the plan, into the
+// caller's tensors (or every rank's bucket).  `grad_scratch_bytes`: the compact-row part of the scratch.
+static int backward_body(GsContext* ctx, const GsFrame* f, const int32_t* radii, const void* geom_buffer,
+                         const void* binning_buffer, int64_t pair_capacity, const void* image_buffer, void* grad_scratch,
+                         size_t grad_scratch_bytes, const float* dL_dout_color, const GsGrads* grads,
+                         const GsDetLayout* det, gs_stream_t stream) {
     int rc = check_frame(f);
     if (rc) return rc;
-    if (f->P == 0) return GS_OK;
-    if (!geom_buffer || !binning_buffer || !image_buffer || !dL_dout_color)
-        return fail(GS_EINVAL, "scratch / dL_dout_color is NULL");
+    if (f->P > 0) {
+        if (!geom_buffer || !binning_buffer || !image_buffer || !dL_dout_color)
+            return fail(GS_EINVAL, "scratch / dL_dout_color is NULL");
+        if (!radii || !grad_scratch) return fail(GS_EINVAL, "radii / scratch is NULL");
+        if (grads->peer_world > GS_MAX_PEERS || (grads->peer_world > 0 && !grads->peer_buckets))
+            return fail(GS_EINVAL, "bad peer arguments");
+    }
     cudaStream_t s = (cudaStream_t)stream;
-    const GsView v = make_view(f);
+    const GsGradPtrs g = grad_ptrs(f, grads);
+    const GradPlan plan = grad_plan(ctx, f, grads, g, (long long)(grad_scratch_bytes / (GS_GOUT_FLOATS * sizeof(float))));
     GsImageLayout il = gs_image_layout(const_cast<void*>(image_buffer), f->W, f->H);
+    if (plan.fill || plan.peer_begin) {
+        if ((rc = ensure_aux(ctx))) return rc;
+        GS_CUDA(cudaEventRecord(ctx->aux_fork, s));        // the outputs were allocated in `stream` order before this call
+        GS_CUDA(cudaStreamWaitEvent(ctx->aux, ctx->aux_fork, 0));
+        // the tile pass is issue bound and leaves the memory system idle; in the dense regime the fill exits on the device
+        if (plan.fill) GS_TIMED(ctx, 11, ctx->aux, gs_launch_fill_zero(f->P, ctx->num_sms, g, il.status, plan.dense_ok, ctx->aux));
+        else gs_launch_peer_barrier((uint32_t* const*)grads->peer_signals, grads->peer_world, grads->peer_rank, 0,
+                                    grads->peer_epoch_begin, ctx->aux);
+        GS_CUDA(cudaEventRecord(ctx->aux_join, ctx->aux));
+    }
+    if (f->P == 0) return GS_OK;
+    const GsView v = make_view(f);
+    const int nsm = ctx ? ctx->num_sms : g_gs_num_sms;
     GsGeomLayout gl = gs_geom_layout(const_cast<void*>(geom_buffer), f->P);
     GsBinLayout bl = gs_bin_layout(const_cast<void*>(binning_buffer), pair_capacity > 0 ? pair_capacity : 1);
-    GS_TIMED(ctx, 6, s, gs_launch_blend_bwd(v, il.tile_off, bl.list, gl.rec, il.final_T, il.n_contrib, dL_dout_color,
-                                            gl.acc, il.status, pair_capacity, s));
-    return debug_sync(f, s, "blend_bwd");
-}
-
-// Backward, per-Gaussian pass: gradients from the accumulators into the caller's tensors (or peers' buckets).
-static int backward_gradients(GsContext* ctx, const GsFrame* f, const int32_t* radii, const void* geom_buffer,
-                          const void* image_buffer, void* grad_scratch, size_t grad_scratch_bytes,
-                          const GsGrads* grads, gs_stream_t stream) {
-    int rc = check_frame(f);
-    if (rc) return rc;
-    if (!grads) return fail(GS_EINVAL, "grads is NULL");
-    if (f->P == 0) return GS_OK;
-    if (!radii || !geom_buffer || !image_buffer || !grad_scratch) return fail(GS_EINVAL, "radii / scratch is NULL");
-    cudaStream_t s = (cudaStream_t)stream;
-    const GsView v = make_view(f);
-    GsImageLayout il = gs_image_layout(const_cast<void*>(image_buffer), f->W, f->H);
-    GsGeomLayout gl = gs_geom_layout(const_cast<void*>(geom_buffer), f->P);
-    const GsGradPtrs g = grad_ptrs(f, grads);
-    float* gout = (float*)grad_scratch;
-    // backward_prefill ran for these outputs: join the side stream, the per-Gaussian kernel scatters final rows
-    const bool prefilled = ctx && ctx->prefilled && ctx->prefilled == (const void*)grads->dL_dsh && grads->peer_world <= 0;
-    if (prefilled) {
-        GS_CUDA(cudaStreamWaitEvent(s, ctx->aux_join, 0));
-        ctx->prefilled = nullptr;
+    if (!det) {
+        GS_TIMED(ctx, 6, s, gs_launch_blend_bwd(v, il.tile_off, bl.list, gl.rec, il.final_T, il.n_contrib, dL_dout_color,
+                                                gl.acc, il.status, pair_capacity, s));
+        if ((rc = debug_sync(f, s, "blend_bwd"))) return rc;
+    } else {
+        gs_launch_tile_partials(v, il.tile_off, bl.list, gl.rec, il.final_T, il.n_contrib, dL_dout_color, det->part_a,
+                                det->part_b, il.status, pair_capacity, s);
+        if ((rc = debug_sync(f, s, "tile_partials"))) return rc;
+        gs_launch_det_reduce(*det, nsm, bl.list, gl.vis_list, gl.acc, il.status, pair_capacity, s);
+        if ((rc = debug_sync(f, s, "det_reduce"))) return rc;
     }
-    // When most Gaussians are visible (decided on the device from num_visible) ONE dense kernel does the whole
-    // per-Gaussian backward and the compact pair below returns at once; otherwise the other way round.  The dense
-    // kernel covers the reference's own input mode (SH degree <= 3 stored as 16 coefficients, scales + rotations).
-    const bool dense_ok = dense_eligible(f, grads, g);
-    GS_TIMED(ctx, 7, s, gs_launch_grad_vis(v, ctx ? ctx->num_sms : g_gs_num_sms, f->means3D, f->shs,
-                                           f->cov3D_precomp ? nullptr : f->scales,
+
+    float* gout = (float*)grad_scratch;
+    if (plan.fill) GS_CUDA(cudaStreamWaitEvent(s, ctx->aux_join, 0));
+    GS_TIMED(ctx, 7, s, gs_launch_grad_vis(v, nsm, f->means3D, f->shs, f->cov3D_precomp ? nullptr : f->scales,
                                            f->cov3D_precomp ? nullptr : f->rotations, f->cov3D_precomp, gl.rec, gl.acc,
-                                           gl.vis_list, il.status, gout, dense_ok, prefilled, g, s));
+                                           gl.vis_list, il.status, gout, plan.dense_ok, plan.fill, g, s));
     if ((rc = debug_sync(f, s, "grad_vis"))) return rc;
-    if (grads->peer_world > 0) {
-        // data-parallel shared-model step: the five parameter gradients are reduced straight into every rank's
-        // bucket (peer stores / NVSwitch multicast); only dL_dmeans2D is written locally
-        if (grads->peer_world > GS_MAX_PEERS || !grads->peer_buckets) return fail(GS_EINVAL, "bad peer arguments");
-        const bool sync = ctx && grads->peer_signals;
-        if (sync && grads->peer_epoch_begin) {
-            // nobody adds into a bucket before every rank has cleared its own: one-warp barrier kernel, normally already
-            // done -- gs_backward put it on the side stream beside the tile pass
-            if (ctx->peer_barrier_pending) GS_CUDA(cudaStreamWaitEvent(s, ctx->aux_join, 0));
-            else gs_launch_peer_barrier((uint32_t* const*)grads->peer_signals, grads->peer_world, grads->peer_rank, 0,
-                                        grads->peer_epoch_begin, s);
-            ctx->peer_barrier_pending = false;
-        }
+    if (plan.peer) {
+        // nobody adds into a bucket before every rank has cleared its own
+        if (plan.peer_begin) GS_CUDA(cudaStreamWaitEvent(s, ctx->aux_join, 0));
         GS_TIMED(ctx, 9, s, gs_launch_grad_reduce_peers(f->P, v.M, radii, gl.acc, gout, grads->dL_dmeans2D,
                                                         (float* const*)grads->peer_buckets, grads->peer_world,
                                                         (float*)grads->peer_multicast, (const long long*)grads->peer_seg_off, s));
         // the step's result is complete on this rank when every rank's adds have landed
-        if (sync && grads->peer_epoch_end)
+        if (ctx && grads->peer_signals && grads->peer_epoch_end)
             gs_launch_peer_barrier((uint32_t* const*)grads->peer_signals, grads->peer_world, grads->peer_rank, 1,
                                    grads->peer_epoch_end, s);
         return debug_sync(f, s, "grad_reduce_peers");
     }
-    if (!prefilled) {
-        GS_TIMED(ctx, 9, s, gs_launch_grad_write(f->P, v.M, radii, gl.acc, gout, g, il.status, dense_ok, s));
+    if (plan.writer != GradWriter::none) {
+        GS_TIMED(ctx, 9, s, gs_launch_grad_write(f->P, v.M, radii, gl.acc, gout, g, il.status, plan.dense_ok,
+                                                 plan.writer == GradWriter::tma, s));
         if ((rc = debug_sync(f, s, "grad_write"))) return rc;
     }
-    // a scratch buffer sized from the true visible count (synchronising hosts) can prove the sparse regime: no launch
-    const long long nvis_bound = (long long)(grad_scratch_bytes / (GS_GOUT_FLOATS * sizeof(float)));
-    if (dense_ok && 2 * nvis_bound > (long long)f->P) {
-        GS_TIMED(ctx, 10, s, gs_launch_grad_dense(v, ctx ? ctx->num_sms : g_gs_num_sms, f->means3D, f->shs, f->scales, f->rotations,
-                                                  radii, gl.acc, il.status, g, s));
+    if (plan.dense) {
+        GS_TIMED(ctx, 10, s, gs_launch_grad_dense(v, nsm, f->means3D, f->shs, f->scales, f->rotations, radii, gl.acc,
+                                                  il.status, g, s));
         if ((rc = debug_sync(f, s, "grad_dense"))) return rc;
     }
     // outputs the fused kernel does not produce in this input mode are defined as zeros (reference: torch::zeros)
@@ -580,22 +563,8 @@ int gs_backward(GsContext* ctx, const GsFrame* f, const int32_t* radii, const vo
                 const GsGrads* grads, gs_stream_t stream) {
     (void)dL_dout_depth;                                 // depth gradient disabled in the reference
     if (!grads) return fail(GS_EINVAL, "grads is NULL");
-    int rc = ctx ? backward_prefill(ctx, f, image_buffer, grads, stream) : GS_OK;
-    if (rc) return rc;
-    if (ctx && grads->peer_world > 0 && grads->peer_signals && grads->peer_epoch_begin) {
-        // shared-model step: the "every bucket is cleared" barrier waits on the side stream while the tile pass runs
-        if ((rc = ensure_aux(ctx))) return rc;
-        cudaStream_t s = (cudaStream_t)stream;
-        GS_CUDA(cudaEventRecord(ctx->aux_fork, s));
-        GS_CUDA(cudaStreamWaitEvent(ctx->aux, ctx->aux_fork, 0));
-        gs_launch_peer_barrier((uint32_t* const*)grads->peer_signals, grads->peer_world, grads->peer_rank, 0,
-                               grads->peer_epoch_begin, ctx->aux);
-        GS_CUDA(cudaEventRecord(ctx->aux_join, ctx->aux));
-        ctx->peer_barrier_pending = true;
-    }
-    rc = backward_blend(ctx, f, geom_buffer, binning_buffer, pair_capacity, image_buffer, dL_dout_color, stream);
-    if (rc) return rc;
-    return backward_gradients(ctx, f, radii, geom_buffer, image_buffer, grad_scratch, grad_scratch_bytes, grads, stream);
+    return backward_body(ctx, f, radii, geom_buffer, binning_buffer, pair_capacity, image_buffer, grad_scratch,
+                         grad_scratch_bytes, dL_dout_color, grads, nullptr, stream);
 }
 
 // Bytes of the deterministic backward's scratch for `num_visible` compact slots and `pair_capacity` pairs: the default
@@ -608,29 +577,9 @@ size_t gs_backward_deterministic_scratch_bytes(int64_t num_visible, int64_t pair
     return det_scratch_bytes(num_visible > 0 ? num_visible : 1, pair_capacity > 0 ? pair_capacity : 1);
 }
 
-// Backward, deterministic tile pass: per-(tile, splat) partials stored by list position, then summed per Gaussian in
-// ascending list position into the accumulators (gs_det_bwd.cu) -- the same accumulator contents as backward_blend up to
+// The deterministic tile pass stores per-(tile, splat) partials by list position and sums them per Gaussian in
+// ascending list position into the accumulators (gs_det_bwd.cu): the same accumulator contents as k_blend_bwd up to
 // the order of the float additions, which is fixed here.
-static int backward_blend_deterministic(GsContext* ctx, const GsFrame* f, const void* geom_buffer, const void* binning_buffer,
-                                        int64_t pair_capacity, const void* image_buffer, const float* dL_dout_color,
-                                        const GsDetLayout& d, gs_stream_t stream) {
-    int rc = check_frame(f);
-    if (rc) return rc;
-    if (f->P == 0) return GS_OK;
-    if (!geom_buffer || !binning_buffer || !image_buffer || !dL_dout_color)
-        return fail(GS_EINVAL, "scratch / dL_dout_color is NULL");
-    cudaStream_t s = (cudaStream_t)stream;
-    const GsView v = make_view(f);
-    GsImageLayout il = gs_image_layout(const_cast<void*>(image_buffer), f->W, f->H);
-    GsGeomLayout gl = gs_geom_layout(const_cast<void*>(geom_buffer), f->P);
-    GsBinLayout bl = gs_bin_layout(const_cast<void*>(binning_buffer), pair_capacity > 0 ? pair_capacity : 1);
-    gs_launch_tile_partials(v, il.tile_off, bl.list, gl.rec, il.final_T, il.n_contrib, dL_dout_color, d.part_a, d.part_b,
-                            il.status, pair_capacity, s);
-    if ((rc = debug_sync(f, s, "tile_partials"))) return rc;
-    gs_launch_det_reduce(d, ctx ? ctx->num_sms : g_gs_num_sms, bl.list, gl.vis_list, gl.acc, il.status, pair_capacity, s);
-    return debug_sync(f, s, "det_reduce");
-}
-
 int gs_backward_deterministic(GsContext* ctx, const GsFrame* f, const int32_t* radii, const void* geom_buffer,
                               const void* binning_buffer, int64_t pair_capacity, const void* image_buffer,
                               void* grad_scratch, size_t grad_scratch_bytes, const float* dL_dout_color,
@@ -654,13 +603,9 @@ int gs_backward_deterministic(GsContext* ctx, const GsFrame* f, const int32_t* r
     const long long V = lo;
     const size_t default_bytes = gs_backward_scratch_bytes(V);
     const GsDetLayout d = gs_det_layout((char*)grad_scratch + default_bytes, V, C);
-    int rc = ctx ? backward_prefill(ctx, f, image_buffer, grads, stream) : GS_OK;
-    if (rc) return rc;
-    rc = backward_blend_deterministic(ctx, f, geom_buffer, binning_buffer, pair_capacity, image_buffer, dL_dout_color, d,
-                                      stream);
-    if (rc) return rc;
-    // backward_gradients bounds the visible count by the size of ITS scratch: the default part only
-    return backward_gradients(ctx, f, radii, geom_buffer, image_buffer, grad_scratch, default_bytes, grads, stream);
+    // the compact rows bound the visible count by the default part of the scratch only
+    return backward_body(ctx, f, radii, geom_buffer, binning_buffer, pair_capacity, image_buffer, grad_scratch,
+                         default_bytes, dL_dout_color, grads, &d, stream);
 }
 
 int gs_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,

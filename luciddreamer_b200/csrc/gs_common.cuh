@@ -362,7 +362,6 @@ void gs_launch_grad_vis(const GsView& v, int num_sms, const float* means3D, cons
                         const float* rotations, const float* cov3D_precomp, const float4* rec, float4* acc,
                         const uint32_t* vis_list, const GsDevStatus* status, float* gout, bool dense_elsewhere,
                         bool scatter, GsGradPtrs g, cudaStream_t s);
-bool gs_grads_tma_ok(int M, const GsGradPtrs& g);
 void gs_launch_fill_zero(int P, int num_sms, const GsGradPtrs& g, const GsDevStatus* status, bool dense_elsewhere,
                          cudaStream_t s);
 void gs_launch_grad_dense(const GsView& v, int num_sms, const float* means3D, const float* shs, const float* scales,
@@ -370,7 +369,7 @@ void gs_launch_grad_dense(const GsView& v, int num_sms, const float* means3D, co
                           cudaStream_t s);
 void gs_grad_write_init();
 void gs_launch_grad_write(int P, int M, const int* radii, const float4* acc, const float* gout, GsGradPtrs g,
-                          const GsDevStatus* status, bool dense_elsewhere, cudaStream_t s);
+                          const GsDevStatus* status, bool dense_elsewhere, bool tma, cudaStream_t s);
 void gs_launch_grad_reduce_peers(int P, int M, const int* radii, const float4* acc, const float* gout, float* dmeans2D,
                                  float* const* peers, int world, float* mc, const long long* seg_off,
                                  cudaStream_t s);

@@ -1,25 +1,82 @@
-// Per-Gaussian backward (sm_90a), two kernels:
+// Per-Gaussian backward (sm_90a): turns the 9-float accumulator rows of the tile pass into the FINAL dense gradient
+// tensors.  Replaces, fused: computeCov2DCUDA (RAST/cuda_rasterizer/backward.cu:144-274), preprocessCUDA bwd (:346-396,
+// with the SH backward :20-139 and the cov3D backward :278-341), the nine torch::zeros fills of the binding
+// (RAST/rasterize_points.cu:154-162) and every read-modify-write the reference does on dense [P,*] intermediates
+// (dL_dconic, dL_dcov3D, dL_dcolors never exist as dense tensors unless the caller asks for them).  Seven kernels:
 //
-//   k_grad_vis    dense over the compact visible list: turns the 9-float accumulator of the tile pass into the
-//                 per-Gaussian gradients.  Replaces, fused: computeCov2DCUDA (RAST/cuda_rasterizer/backward.cu:
-//                 144-274) and preprocessCUDA bwd (:346-396, with the SH backward :20-139 and the cov3D backward
-//                 :278-341).  Result: one 44-float row per visible Gaussian in a compact scratch buffer (the
-//                 dL_dsh block is kept factored as basis[16] x dRGB[3]).
-//   k_grad_write  streaming over all P rows: expands / copies the compact rows into the FINAL dense gradient
-//                 tensors and writes zeros for invisible Gaussians.  Replaces the nine torch::zeros fills of the
-//                 binding (RAST/rasterize_points.cu:154-162) and every read-modify-write the reference does on
-//                 dense [P,*] intermediates (dL_dconic, dL_dcov3D, dL_dcolors never exist as dense tensors unless
-//                 the caller asks for them).  HBM-bound: ~248 B written + 4 B read per Gaussian; every store is a
-//                 fully coalesced 128-bit (dL_dsh, rotations) or 32-bit row-contiguous store.
+//   k_grad_vis           over the compact visible list: one 44-float compact row per visible Gaussian in the scratch
+//                        (the dL_dsh block kept factored as basis[16] x dRGB[3]), or, after k_fill_zero, the final rows
+//                        scattered straight into the outputs
+//   k_fill_zero          zeroes the six outputs by TMA on a side stream, beside the tile pass
+//   k_grad_write         streaming over all P rows: expands the compact rows into the outputs, zeros for invisible rows
+//   k_grad_write_tma     the same for the reference's own input mode, each block assembled in shared memory and stored
+//                        by TMA
+//   k_grad_dense         more than half of the Gaussians visible: the whole per-Gaussian backward in one TMA pipeline
+//   k_grad_reduce_peers  data-parallel shared-model step: adds the visible rows into every rank's bucket
+//   k_peer_barrier       that step's cross-rank barrier
+//
+// Routes, chosen once per call by grad_plan (gs_api.cu); "six outputs" = exactly the six gradients of the reference's
+// input mode (16 stored SH coefficients), 16-byte aligned:
+//   six outputs, scales + rotations, P % 4 = 0, a context   k_fill_zero + k_grad_vis scattering
+//   six outputs otherwise                                    k_grad_vis + k_grad_write_tma
+//   any other outputs                                        k_grad_vis + k_grad_write
+//   peer reduce                                 [k_peer_barrier] k_grad_vis + k_grad_reduce_peers [k_peer_barrier]
+// With six outputs, scales + rotations and no peer reduce, k_grad_dense is launched as well unless the scratch proves
+// the sparse regime; the device decides from num_visible which of it and the sparse kernels does the work, and the
+// others return at once.
 
 #include "gs_common.cuh"
 
 namespace {
 
 constexpr int kT = 256;
-// compact gradient row (floats): 0-2 dmean3D, 3-4 dmean2D, 5 dopacity, 6-8 dscale, 9-12 drot, 13-15 dRGB (clamp
-// masked), 16-31 SH basis, 32-34 dcolor (raw), 35-40 dcov3D, 41-43 pad
+// compact gradient row (floats), 11 float4: dmean3D[3], dmean2D[2], dopacity, dscale[3], drot[4], dRGB[3] (clamp
+// masked), SH basis[16], dcolor[3] (raw), dcov3D[6], 3 floats of padding
 constexpr int kRow = GS_GOUT_FLOATS;
+struct Row {
+    static constexpr int dmean3D = 0, dmean2D = 3, dopacity = 5, dscale = 6, drot = 9, dRGB = 13, basis = 16, dcolor = 32,
+                         dcov3D = 35;
+};
+
+// The accumulator row of one Gaussian (a0, a1, a2, read from `src`: the row itself or a staged copy of it), re-armed in
+// `aa` for the next backward: zeros, keeping the clamp bits (a2.y) and the compact slot (a2.w).
+__device__ __forceinline__ void take_acc(float4* aa, const float4* src, float4& a0, float4& a1, float4& a2) {
+    a0 = src[0]; a1 = src[1]; a2 = src[2];
+    const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    aa[0] = z4; aa[1] = z4; aa[2] = make_float4(0.f, a2.y, 0.f, a2.w);
+}
+
+// Row i of the six dense outputs from a finished compact row o: dL_dmeans3D, dL_dmeans2D (its third component is zero,
+// stored when kM2z), dL_dopacity, dL_dscales, dL_drotations and dL_dsh = basis x dRGB (16 coefficients).  The
+// destinations are global memory or a shared-memory image of a block.  kVec: dL_drotations and dL_dsh leave as float4
+// (16-byte aligned rows), else as scalars.  I is the caller's index type, which shapes the address arithmetic.
+template <bool kVec, bool kM2z, typename I>
+__device__ __forceinline__ void expand_row(const float4* o, float* m3, float* m2, float* op, float* sc, float* rot,
+                                           float* sh, const I i) {
+    m3[3 * i] = o[0].x; m3[3 * i + 1] = o[0].y; m3[3 * i + 2] = o[0].z;
+    m2[3 * i] = o[0].w; m2[3 * i + 1] = o[1].x;
+    if (kM2z) m2[3 * i + 2] = 0.f;
+    op[i] = o[1].y;
+    sc[3 * i] = o[1].z; sc[3 * i + 1] = o[1].w; sc[3 * i + 2] = o[2].x;
+    const float bs[16] = {o[4].x, o[4].y, o[4].z, o[4].w, o[5].x, o[5].y, o[5].z, o[5].w,
+                          o[6].x, o[6].y, o[6].z, o[6].w, o[7].x, o[7].y, o[7].z, o[7].w};
+    const float dR[3] = {o[3].y, o[3].z, o[3].w};
+    if (kVec) {
+        reinterpret_cast<float4*>(rot)[i] = make_float4(o[2].y, o[2].z, o[2].w, o[3].x);
+        float4* d4 = reinterpret_cast<float4*>(sh + (size_t)i * 48);
+#pragma unroll
+        for (int j = 0; j < 12; j++) {
+            float w[4];
+#pragma unroll
+            for (int u = 0; u < 4; u++) { const int e = 4 * j + u; w[u] = bs[e / 3] * dR[e % 3]; }
+            d4[j] = make_float4(w[0], w[1], w[2], w[3]);
+        }
+    } else {
+        rot[4 * i] = o[2].y; rot[4 * i + 1] = o[2].z; rot[4 * i + 2] = o[2].w; rot[4 * i + 3] = o[3].x;
+#pragma unroll
+        for (int e = 0; e < 48; e++) sh[i * 48 + e] = bs[e / 3] * dR[e % 3];
+    }
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void tma_store(void* dst, uint32_t src, uint32_t bytes) {
@@ -236,10 +293,8 @@ k_grad_vis(const GsView v, const float* __restrict__ means3D, const float* __res
     const uint32_t nvis = (uint32_t)status->num_visible;
     for (uint32_t c = blockIdx.x * kVisT + threadIdx.x; c < nvis; c += gridDim.x * kVisT) {
         const uint32_t i = vis_list[c];
-        float4* aa = acc + (size_t)3 * i;
-        const float4 a0 = aa[0], a1 = aa[1], a2 = aa[2];
-        const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        aa[0] = z4; aa[1] = z4; aa[2] = make_float4(0.f, a2.y, 0.f, a2.w);  // re-arm; keep the clamp bits + compact slot
+        float4 a0, a1, a2;
+        take_acc(acc + (size_t)3 * i, acc + (size_t)3 * i, a0, a1, a2);
         const uint32_t clamped = __float_as_uint(a2.y);
         const float* sh = shs ? shs + (size_t)i * v.M * 3 : nullptr;
         // 128-bit loads when the rows are 16-byte aligned (M * 3 a multiple of 4, base aligned like every input --
@@ -267,22 +322,7 @@ k_grad_vis(const GsView v, const float* __restrict__ means3D, const float* __res
         // the dense outputs were zero-filled beside the tile pass (k_fill_zero): the final rows go straight into them
         float4 o[11];
         grad_row(v, cam, i, a0, a1, a2, clamped, means3D, true, scales, rotations, cov3D_precomp, fill, o);
-        g.dmeans3D[3 * i] = o[0].x; g.dmeans3D[3 * i + 1] = o[0].y; g.dmeans3D[3 * i + 2] = o[0].z;
-        g.dmeans2D[3 * i] = o[0].w; g.dmeans2D[3 * i + 1] = o[1].x;
-        g.dopacity[i] = o[1].y;
-        g.dscales[3 * i] = o[1].z; g.dscales[3 * i + 1] = o[1].w; g.dscales[3 * i + 2] = o[2].x;
-        reinterpret_cast<float4*>(g.drots)[i] = make_float4(o[2].y, o[2].z, o[2].w, o[3].x);
-        const float bs[16] = {o[4].x, o[4].y, o[4].z, o[4].w, o[5].x, o[5].y, o[5].z, o[5].w,
-                              o[6].x, o[6].y, o[6].z, o[6].w, o[7].x, o[7].y, o[7].z, o[7].w};
-        const float dR[3] = {o[3].y, o[3].z, o[3].w};
-        float4* d4 = reinterpret_cast<float4*>(g.dsh + (size_t)i * 48);
-#pragma unroll
-        for (int j = 0; j < 12; j++) {
-            float w[4];
-#pragma unroll
-            for (int u = 0; u < 4; u++) { const int e = 4 * j + u; w[u] = bs[e / 3] * dR[e % 3]; }
-            d4[j] = make_float4(w[0], w[1], w[2], w[3]);
-        }
+        expand_row<true, false>(o, g.dmeans3D, g.dmeans2D, g.dopacity, g.dscales, g.drots, g.dsh, i);   // the fill left dmeans2D[.][2] zero
     }
 }
 
@@ -344,7 +384,6 @@ __device__ __forceinline__ void cta_zero_run(float* __restrict__ base, long long
     }
 }
 
-// `cl` = s_slot[threadIdx.x]; `count` = number of visible rows of the CTA
 // One run of zeros by TMA: `bytes` (a multiple of 16) from the 16 KB zero buffer in shared memory, 16 KB at a time.
 __device__ __forceinline__ bool tma_zero_run(float* base, long long row0, int nf, int rows, uint32_t zsrc) {
     if (!base || nf <= 0) return true;
@@ -356,6 +395,7 @@ __device__ __forceinline__ bool tma_zero_run(float* base, long long row0, int nf
     return true;
 }
 
+// `cl` = s_slot[threadIdx.x]; `count` = number of visible rows of the CTA
 template <int NT, int RS>
 __device__ __forceinline__ void cta_write_block(const int P, const int M, const long long row0, const float* s_row,
                                                 const int* s_slot, const int cl, const int count, const GsGradPtrs& g,
@@ -395,7 +435,7 @@ __device__ __forceinline__ void cta_write_block(const int P, const int M, const 
         cta_zero_run<NT>(g.drots, row0, 4);    cta_zero_run<NT>(g.dsh, row0, M3z);
         return;
     }
-    if (g.dmeans3D) cta_store_rows<3, NT, RS>(g.dmeans3D, s_row, s_slot, 0, row0, P);
+    if (g.dmeans3D) cta_store_rows<3, NT, RS>(g.dmeans3D, s_row, s_slot, Row::dmean3D, row0, P);
     if (g.dmeans2D) {
         const long long base = row0 * 3, lim = (long long)P * 3;
 #pragma unroll
@@ -403,17 +443,17 @@ __device__ __forceinline__ void cta_write_block(const int P, const int M, const 
             const int e = tid + NT * k;
             const int row = e / 3, comp = e - row * 3;
             const int c2 = s_slot[row];
-            if (base + e < lim) g.dmeans2D[base + e] = (c2 < 0 || comp == 2) ? 0.f : s_row[c2 * RS + 3 + comp];
+            if (base + e < lim) g.dmeans2D[base + e] = (c2 < 0 || comp == 2) ? 0.f : s_row[c2 * RS + Row::dmean2D + comp];
         }
     }
-    if (g.dscales) cta_store_rows<3, NT, RS>(g.dscales, s_row, s_slot, 6, row0, P);
-    if (g.dcolors) cta_store_rows<3, NT, RS>(g.dcolors, s_row, s_slot, 32, row0, P);
-    if (g.dcov3D) cta_store_rows<6, NT, RS>(g.dcov3D, s_row, s_slot, 35, row0, P);
+    if (g.dscales) cta_store_rows<3, NT, RS>(g.dscales, s_row, s_slot, Row::dscale, row0, P);
+    if (g.dcolors) cta_store_rows<3, NT, RS>(g.dcolors, s_row, s_slot, Row::dcolor, row0, P);
+    if (g.dcov3D) cta_store_rows<6, NT, RS>(g.dcov3D, s_row, s_slot, Row::dcov3D, row0, P);
     if (i < P) {
-        if (g.dopacity) g.dopacity[i] = cl < 0 ? 0.f : s_row[cl * RS + 5];
+        if (g.dopacity) g.dopacity[i] = cl < 0 ? 0.f : s_row[cl * RS + Row::dopacity];
         if (g.drots) {
             float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (cl >= 0) { const float* q = s_row + cl * RS + 9; r = make_float4(q[0], q[1], q[2], q[3]); }
+            if (cl >= 0) { const float* q = s_row + cl * RS + Row::drot; r = make_float4(q[0], q[1], q[2], q[3]); }
             if ((reinterpret_cast<uintptr_t>(g.drots) & 15) == 0) reinterpret_cast<float4*>(g.drots)[i] = r;
             else { float* d = g.drots + 4 * i; d[0] = r.x; d[1] = r.y; d[2] = r.z; d[3] = r.w; }
         }
@@ -430,8 +470,8 @@ __device__ __forceinline__ void cta_write_block(const int P, const int M, const 
                 const int c2 = s_slot[row];
                 float4 o4 = make_float4(0.f, 0.f, 0.f, 0.f);
                 if (c2 >= 0) {
-                    const float* sb = s_row + c2 * RS + 16;
-                    const float* sr = s_row + c2 * RS + 13;
+                    const float* sb = s_row + c2 * RS + Row::basis;
+                    const float* sr = s_row + c2 * RS + Row::dRGB;
                     float o[4];
 #pragma unroll
                     for (int u = 0; u < 4; u++) {
@@ -448,10 +488,43 @@ __device__ __forceinline__ void cta_write_block(const int P, const int M, const 
                 const int row = e / M3, rem = e - row * M3;
                 const int k = rem / 3, ch = rem - 3 * k;
                 const int c2 = s_slot[row];
-                dst[e] = (c2 < 0 || k >= 16) ? 0.f : s_row[c2 * RS + 16 + k] * s_row[c2 * RS + 13 + ch];
+                dst[e] = (c2 < 0 || k >= 16) ? 0.f : s_row[c2 * RS + Row::basis + k] * s_row[c2 * RS + Row::dRGB + ch];
             }
         }
     }
+}
+
+// The kT rows [row0, row0 + kT) of one CTA: every visible row claims a CTA-local compact slot (s_slot[row], -1 for an
+// invisible row; *s_count = visible rows; s_rowidx[slot] = row when kRowIdx) and stages its compact row (k_grad_vis) at
+// s_row + slot * kRow.  Returns the calling thread's slot; the CTA is synchronised on return.
+template <bool kRowIdx>
+__device__ __forceinline__ int claim_and_stage(const int P, const int* __restrict__ radii, const float4* __restrict__ acc,
+                                               const float* __restrict__ gout, const long long row0, float* s_row,
+                                               int* s_slot, int* s_count, int* s_rowidx) {
+    const int tid = threadIdx.x, lane = tid & 31;
+    const long long i = row0 + tid;
+    if (tid == 0) *s_count = 0;
+    __syncthreads();
+    const bool vis = i < P && radii[i] > 0;
+    const unsigned m = __ballot_sync(0xffffffffu, vis);
+    int cl = -1;
+    if (m) {
+        int base = 0;
+        if (lane == __ffs(m) - 1) base = atomicAdd(s_count, __popc(m));
+        base = __shfl_sync(0xffffffffu, base, __ffs(m) - 1);
+        if (vis) cl = base + __popc(m & ((1u << lane) - 1u));
+    }
+    s_slot[tid] = cl;
+    if (vis) {
+        if (kRowIdx) s_rowidx[cl] = tid;
+        const uint32_t slot = __float_as_uint(__ldg(reinterpret_cast<const float*>(acc + (size_t)3 * i + 2) + 3));
+        const float4* src = reinterpret_cast<const float4*>(gout + (size_t)slot * kRow);
+        float4* dstr = reinterpret_cast<float4*>(s_row + cl * kRow);
+#pragma unroll
+        for (int k = 0; k < kRow / 4; k++) dstr[k] = __ldg(src + k);
+    }
+    __syncthreads();
+    return cl;
 }
 
 __global__ void __launch_bounds__(kT)
@@ -462,29 +535,8 @@ k_grad_write(const int P, const int M, const int* __restrict__ radii, const floa
     extern __shared__ __align__(16) float s_row[];       // kT * kRow floats: staged compact rows of this CTA
     __shared__ int s_slot[kT];
     __shared__ int s_count;
-    const int tid = threadIdx.x, lane = tid & 31;
     const long long row0 = (long long)blockIdx.x * kT;
-    const long long i = row0 + tid;
-    if (tid == 0) s_count = 0;
-    __syncthreads();
-    const bool vis = i < P && radii[i] > 0;
-    const unsigned m = __ballot_sync(0xffffffffu, vis);
-    int cl = -1;
-    if (m) {
-        int base = 0;
-        if (lane == __ffs(m) - 1) base = atomicAdd(&s_count, __popc(m));
-        base = __shfl_sync(0xffffffffu, base, __ffs(m) - 1);
-        if (vis) cl = base + __popc(m & ((1u << lane) - 1u));
-    }
-    s_slot[tid] = cl;
-    if (vis) {
-        const uint32_t slot = __float_as_uint(__ldg(reinterpret_cast<const float*>(acc + (size_t)3 * i + 2) + 3));
-        const float4* src = reinterpret_cast<const float4*>(gout + (size_t)slot * kRow);
-        float4* dstr = reinterpret_cast<float4*>(s_row + cl * kRow);
-#pragma unroll
-        for (int k = 0; k < kRow / 4; k++) dstr[k] = __ldg(src + k);
-    }
-    __syncthreads();
+    const int cl = claim_and_stage<false>(P, radii, acc, gout, row0, s_row, s_slot, &s_count, nullptr);
     cta_write_block<kT, kRow>(P, M, row0, s_row, s_slot, cl, s_count, g, s_row);   // s_row doubles as the zero buffer
 }
 
@@ -519,11 +571,11 @@ k_grad_write_tma(const int P, const int* __restrict__ radii, const float4* __res
 #pragma unroll
         for (int k = 0; k < 11; k++) o[k] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    const float bs[16] = {o[4].x, o[4].y, o[4].z, o[4].w, o[5].x, o[5].y, o[5].z, o[5].w,
-                          o[6].x, o[6].y, o[6].z, o[6].w, o[7].x, o[7].y, o[7].z, o[7].w};
-    const float dR[3] = {o[3].y, o[3].z, o[3].w};
     if (full) {
         // every thread writes its own row of every tensor (zeros for an invisible row): conflict-free, no second pass
+        const float bs[16] = {o[4].x, o[4].y, o[4].z, o[4].w, o[5].x, o[5].y, o[5].z, o[5].w,
+                              o[6].x, o[6].y, o[6].z, o[6].w, o[7].x, o[7].y, o[7].z, o[7].w};
+        const float dR[3] = {o[3].y, o[3].z, o[3].w};
         float4* d4 = reinterpret_cast<float4*>(img + WriteImg::sh) + tid * 12;
 #pragma unroll
         for (int j = 0; j < 12; j++) {
@@ -556,15 +608,8 @@ k_grad_write_tma(const int P, const int* __restrict__ radii, const float4* __res
         __syncthreads();
         continue;
     }
-    if (i < P) {                                           // last, partial block: plain stores
-        g.dmeans3D[3 * i] = o[0].x; g.dmeans3D[3 * i + 1] = o[0].y; g.dmeans3D[3 * i + 2] = o[0].z;
-        g.dmeans2D[3 * i] = o[0].w; g.dmeans2D[3 * i + 1] = o[1].x; g.dmeans2D[3 * i + 2] = 0.f;
-        g.dopacity[i] = o[1].y;
-        g.dscales[3 * i] = o[1].z; g.dscales[3 * i + 1] = o[1].w; g.dscales[3 * i + 2] = o[2].x;
-        g.drots[4 * i] = o[2].y; g.drots[4 * i + 1] = o[2].z; g.drots[4 * i + 2] = o[2].w; g.drots[4 * i + 3] = o[3].x;
-#pragma unroll
-        for (int e = 0; e < 48; e++) g.dsh[i * 48 + e] = bs[e / 3] * dR[e % 3];
-    }
+    if (i < P)                                             // last, partial block: plain stores
+        expand_row<false, true>(o, g.dmeans3D, g.dmeans2D, g.dopacity, g.dscales, g.drots, g.dsh, i);
   }
 }
 
@@ -646,11 +691,8 @@ k_grad_dense(const GsView v, const float* __restrict__ means3D, const float* __r
         float* s_dop = reinterpret_cast<float*>(S + DenseStage::dop) + tid;
         float4 o[11];
         if (vis) {
-            const float4* sa = reinterpret_cast<const float4*>(S + DenseStage::acc) + tid * 3;
-            const float4 a0 = sa[0], a1 = sa[1], a2 = sa[2];
-            float4* aa = acc + i * 3;
-            const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            aa[0] = z4; aa[1] = z4; aa[2] = make_float4(0.f, a2.y, 0.f, a2.w);  // re-arm; keep the clamp bits + compact slot
+            float4 a0, a1, a2;
+            take_acc(acc + i * 3, reinterpret_cast<const float4*>(S + DenseStage::acc) + tid * 3, a0, a1, a2);
             const float3 p = make_float3(s_m[0], s_m[1], s_m[2]);
             const float3 sc = make_float3(s_s[0], s_s[1], s_s[2]);
             const float4 q = *s_r;
@@ -669,24 +711,7 @@ k_grad_dense(const GsView v, const float* __restrict__ means3D, const float* __r
             for (int k = 0; k < 11; k++) o[k] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
         // every thread writes only slots it alone read: its SH row, mean, scale, rotation (dm2 / dop have their own)
-        s_m[0] = o[0].x; s_m[1] = o[0].y; s_m[2] = o[0].z;                       // dL_dmeans3D
-        s_dm2[0] = o[0].w; s_dm2[1] = o[1].x; s_dm2[2] = 0.f;                    // dL_dmeans2D
-        *s_dop = o[1].y;                                                         // dL_dopacity
-        s_s[0] = o[1].z; s_s[1] = o[1].w; s_s[2] = o[2].x;                       // dL_dscales
-        *s_r = make_float4(o[2].y, o[2].z, o[2].w, o[3].x);                      // dL_drotations
-        {
-            const float bs[16] = {o[4].x, o[4].y, o[4].z, o[4].w, o[5].x, o[5].y, o[5].z, o[5].w,
-                                  o[6].x, o[6].y, o[6].z, o[6].w, o[7].x, o[7].y, o[7].z, o[7].w};
-            const float dR[3] = {o[3].y, o[3].z, o[3].w};
-            float4* d4 = reinterpret_cast<float4*>(s_sh);                        // dL_dsh row = basis x dRGB
-#pragma unroll
-            for (int j = 0; j < 12; j++) {
-                float w[4];
-#pragma unroll
-                for (int u = 0; u < 4; u++) { const int e = 4 * j + u; w[u] = bs[e / 3] * dR[e % 3]; }
-                d4[j] = make_float4(w[0], w[1], w[2], w[3]);
-            }
-        }
+        expand_row<true, true>(o, s_m, s_dm2, s_dop, s_s, reinterpret_cast<float*>(s_r), s_sh, 0);
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");             // generic writes -> visible to the TMA
         __syncthreads();
         if (tid == 0) {
@@ -708,10 +733,8 @@ k_grad_dense(const GsView v, const float* __restrict__ means3D, const float* __r
         if (i < (size_t)v.P) {
             float4 o[11];
             if (radii[i] > 0) {
-                float4* aa = acc + i * 3;
-                const float4 a0 = aa[0], a1 = aa[1], a2 = aa[2];
-                const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-                aa[0] = z4; aa[1] = z4; aa[2] = make_float4(0.f, a2.y, 0.f, a2.w);
+                float4 a0, a1, a2;
+                take_acc(acc + i * 3, acc + i * 3, a0, a1, a2);
                 const float* sh = shs + i * 48;
                 auto fill = [&](float* cf, int) {
 #pragma unroll
@@ -722,16 +745,7 @@ k_grad_dense(const GsView v, const float* __restrict__ means3D, const float* __r
 #pragma unroll
                 for (int k = 0; k < 11; k++) o[k] = make_float4(0.f, 0.f, 0.f, 0.f);
             }
-            g.dmeans3D[3 * i] = o[0].x; g.dmeans3D[3 * i + 1] = o[0].y; g.dmeans3D[3 * i + 2] = o[0].z;
-            g.dmeans2D[3 * i] = o[0].w; g.dmeans2D[3 * i + 1] = o[1].x; g.dmeans2D[3 * i + 2] = 0.f;
-            g.dopacity[i] = o[1].y;
-            g.dscales[3 * i] = o[1].z; g.dscales[3 * i + 1] = o[1].w; g.dscales[3 * i + 2] = o[2].x;
-            g.drots[4 * i] = o[2].y; g.drots[4 * i + 1] = o[2].z; g.drots[4 * i + 2] = o[2].w; g.drots[4 * i + 3] = o[3].x;
-            const float bs[16] = {o[4].x, o[4].y, o[4].z, o[4].w, o[5].x, o[5].y, o[5].z, o[5].w,
-                                  o[6].x, o[6].y, o[6].z, o[6].w, o[7].x, o[7].y, o[7].z, o[7].w};
-            const float dR[3] = {o[3].y, o[3].z, o[3].w};
-#pragma unroll
-            for (int e = 0; e < 48; e++) g.dsh[i * 48 + e] = bs[e / 3] * dR[e % 3];
+            expand_row<false, true>(o, g.dmeans3D, g.dmeans2D, g.dopacity, g.dscales, g.drots, g.dsh, i);
         }
     }
 }
@@ -793,30 +807,9 @@ k_grad_reduce_peers(const int P, const int M, const int* __restrict__ radii, con
     __shared__ int s_rowidx[kT];
     __shared__ int s_slot[kT];
     __shared__ int s_count;
-    const int tid = threadIdx.x, lane = tid & 31;
+    const int tid = threadIdx.x;
     const long long row0 = (long long)blockIdx.x * kT;
-    const long long i = row0 + tid;
-    if (tid == 0) s_count = 0;
-    __syncthreads();
-    const bool vis = i < P && radii[i] > 0;
-    const unsigned m = __ballot_sync(0xffffffffu, vis);
-    int cl = -1;
-    if (m) {
-        int base = 0;
-        if (lane == __ffs(m) - 1) base = atomicAdd(&s_count, __popc(m));
-        base = __shfl_sync(0xffffffffu, base, __ffs(m) - 1);
-        if (vis) cl = base + __popc(m & ((1u << lane) - 1u));
-    }
-    s_slot[tid] = cl;
-    if (vis) {
-        s_rowidx[cl] = tid;
-        const uint32_t slot = __float_as_uint(__ldg(reinterpret_cast<const float*>(acc + (size_t)3 * i + 2) + 3));
-        const float4* src = reinterpret_cast<const float4*>(gout + (size_t)slot * kRow);
-        float4* dstr = reinterpret_cast<float4*>(s_row + cl * kRow);
-#pragma unroll
-        for (int k = 0; k < kRow / 4; k++) dstr[k] = __ldg(src + k);
-    }
-    __syncthreads();
+    claim_and_stage<true>(P, radii, acc, gout, row0, s_row, s_slot, &s_count, s_rowidx);
     if (dmeans2D) {                                      // local, dense (zeros for invisible rows)
         const long long base = row0 * 3, lim = (long long)P * 3;
 #pragma unroll
@@ -824,7 +817,7 @@ k_grad_reduce_peers(const int P, const int M, const int* __restrict__ radii, con
             const int e = tid + kT * k;
             const int row = e / 3, comp = e - row * 3;
             const int c2 = s_slot[row];
-            if (base + e < lim) dmeans2D[base + e] = (c2 < 0 || comp == 2) ? 0.f : s_row[c2 * kRow + 3 + comp];
+            if (base + e < lim) dmeans2D[base + e] = (c2 < 0 || comp == 2) ? 0.f : s_row[c2 * kRow + Row::dmean2D + comp];
         }
     }
     const int nv = s_count;
@@ -853,7 +846,7 @@ __device__ __forceinline__ void peer_reduce_rows(const GsPeerArgs& pa, const flo
             const int c2 = e / 20, k = e - c2 * 20;
             const long long gi = row0 + s_rowidx[c2];
             const float* r = s_row + c2 * kRow;
-            if (k < 3) peer_add(pa, pa.off_m3 + gi * 3 + k, r[k]);
+            if (k < 3) peer_add(pa, pa.off_m3 + gi * 3 + k, r[Row::dmean3D + k]);
             else if (k < 15) {
                 const int j = k - 3;                     // float4 j of the row's 48 SH gradients
                 float o[4];
@@ -861,12 +854,12 @@ __device__ __forceinline__ void peer_reduce_rows(const GsPeerArgs& pa, const flo
                 for (int u = 0; u < 4; u++) {
                     const int q = 4 * j + u;
                     const int kk = q / 3, ch = q - 3 * kk;
-                    o[u] = r[16 + kk] * r[13 + ch];
+                    o[u] = r[Row::basis + kk] * r[Row::dRGB + ch];
                 }
                 peer_add4(pa, pa.off_sh + gi * 48 + 4 * j, make_float4(o[0], o[1], o[2], o[3]));
-            } else if (k == 15) peer_add(pa, pa.off_op + gi, r[5]);
-            else if (k < 19) peer_add(pa, pa.off_sc + gi * 3 + (k - 16), r[6 + (k - 16)]);
-            else peer_add4(pa, pa.off_rot + gi * 4, make_float4(r[9], r[10], r[11], r[12]));
+            } else if (k == 15) peer_add(pa, pa.off_op + gi, r[Row::dopacity]);
+            else if (k < 19) peer_add(pa, pa.off_sc + gi * 3 + (k - 16), r[Row::dscale + (k - 16)]);
+            else peer_add4(pa, pa.off_rot + gi * 4, make_float4(r[Row::drot], r[Row::drot + 1], r[Row::drot + 2], r[Row::drot + 3]));
         }
         return;
     }
@@ -876,19 +869,19 @@ __device__ __forceinline__ void peer_reduce_rows(const GsPeerArgs& pa, const flo
         int k = e - c2 * per;
         const long long gi = row0 + s_rowidx[c2];
         const float* r = s_row + c2 * kRow;
-        if (k < 3) { peer_add(pa, pa.off_m3 + gi * 3 + k, r[k]); continue; }
+        if (k < 3) { peer_add(pa, pa.off_m3 + gi * 3 + k, r[Row::dmean3D + k]); continue; }
         k -= 3;
         if (k < M3) {
             const int kk = k / 3, ch = k - 3 * kk;
-            peer_add(pa, pa.off_sh + gi * M3 + k, kk < 16 ? r[16 + kk] * r[13 + ch] : 0.f);
+            peer_add(pa, pa.off_sh + gi * M3 + k, kk < 16 ? r[Row::basis + kk] * r[Row::dRGB + ch] : 0.f);
             continue;
         }
         k -= M3;
-        if (k < 1) { peer_add(pa, pa.off_op + gi, r[5]); continue; }
+        if (k < 1) { peer_add(pa, pa.off_op + gi, r[Row::dopacity]); continue; }
         k -= 1;
-        if (k < 3) { peer_add(pa, pa.off_sc + gi * 3 + k, r[6 + k]); continue; }
+        if (k < 3) { peer_add(pa, pa.off_sc + gi * 3 + k, r[Row::dscale + k]); continue; }
         k -= 3;
-        peer_add(pa, pa.off_rot + gi * 4 + k, r[9 + k]);
+        peer_add(pa, pa.off_rot + gi * 4 + k, r[Row::drot + k]);
     }
 }
 
@@ -926,13 +919,6 @@ void gs_launch_grad_vis(const GsView& v, int num_sms, const float* means3D, cons
     k_grad_vis<<<grid, kVisT, 0, s>>>(v, means3D, shs, scales, rotations, cov3D_precomp, rec, acc, vis_list, status, gout,
                                       dense_elsewhere, scatter, g);
 }
-// true when the outputs qualify for the TMA paths (k_grad_write_tma / k_fill_zero + scatter): the reference's own input
-// mode (16 stored SH coefficients, scales + rotations), all six tensors wanted, 16-byte aligned
-bool gs_grads_tma_ok(int M, const GsGradPtrs& g) {
-    auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
-    return M == 16 && g.dsh && g.dmeans3D && g.dmeans2D && g.dscales && g.dopacity && g.drots && !g.dcolors && !g.dcov3D &&
-           al16(g.dsh) && al16(g.dmeans3D) && al16(g.dmeans2D) && al16(g.dscales) && al16(g.dopacity) && al16(g.drots);
-}
 void gs_launch_fill_zero(int P, int num_sms, const GsGradPtrs& g, const GsDevStatus* status, bool dense_elsewhere,
                          cudaStream_t s) {
     FillRuns r;
@@ -957,9 +943,10 @@ void gs_grad_write_init() {
     cudaFuncSetAttribute(k_grad_reduce_peers, cudaFuncAttributeMaxDynamicSharedMemorySize, kT * kRow * (int)sizeof(float));
     cudaFuncSetAttribute(k_grad_dense, cudaFuncAttributeMaxDynamicSharedMemorySize, kDenseSmem);
 }
+// tma: k_grad_write_tma (the six tensors of the reference's input mode, 16-byte aligned), else the generic k_grad_write
 void gs_launch_grad_write(int P, int M, const int* radii, const float4* acc, const float* gout, GsGradPtrs g,
-                          const GsDevStatus* status, bool dense_elsewhere, cudaStream_t s) {
-    if (gs_grads_tma_ok(M, g)) {
+                          const GsDevStatus* status, bool dense_elsewhere, bool tma, cudaStream_t s) {
+    if (tma) {
         const int need = (P + kWT - 1) / kWT;
         k_grad_write_tma<<<need < g_gs_num_sms * 7 * 2 ? need : g_gs_num_sms * 7 * 2, kWT, 0, s>>>(P, radii, acc, gout, g, status, dense_elsewhere);
         return;

@@ -56,6 +56,18 @@ CASES_ALL = CASES + EXTRA_CASES
 BY_NAME = {c.name: c for c in CASES_ALL}
 
 
+def cov3D_of(scales: torch.Tensor, rotations: torch.Tensor) -> torch.Tensor:
+    """[P, 6] upper triangle of R diag(s^2) R^T, computed in float64 and rounded to float32."""
+    q = rotations.double(); s = scales.double()
+    r, x, y, z = q[:, 0], q[:, 1], q[:, 2], q[:, 3]
+    R = torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - r * z), 2 * (x * z + r * y),
+                     2 * (x * y + r * z), 1 - 2 * (x * x + z * z), 2 * (y * z - r * x),
+                     2 * (x * z - r * y), 2 * (y * z + r * x), 1 - 2 * (x * x + y * y)], -1).reshape(-1, 3, 3)
+    Sg = R @ torch.diag_embed(s * s) @ R.transpose(1, 2)
+    return torch.stack([Sg[:, 0, 0], Sg[:, 0, 1], Sg[:, 0, 2], Sg[:, 1, 1], Sg[:, 1, 2], Sg[:, 2, 2]],
+                       -1).float().contiguous()
+
+
 def build_inputs(case: Case) -> Dict[str, object]:
     """CPU float32 tensors + camera in the reference binding's vocabulary."""
     if case.scene == "frustum":
@@ -83,14 +95,7 @@ def build_inputs(case: Case) -> Dict[str, object]:
         # colours and covariances computed here in plain torch (float64 -> float32): any valid input will do
         g = torch.Generator().manual_seed(case.seed + 99)
         out["colors_precomp"] = torch.rand(case.P, 3, generator=g).contiguous()
-        q = sc["rotations"].double(); s = sc["scales"].double()
-        r, x, y, z = q[:, 0], q[:, 1], q[:, 2], q[:, 3]
-        R = torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - r * z), 2 * (x * z + r * y),
-                         2 * (x * y + r * z), 1 - 2 * (x * x + z * z), 2 * (y * z - r * x),
-                         2 * (x * z - r * y), 2 * (y * z + r * x), 1 - 2 * (x * x + y * y)], -1).reshape(-1, 3, 3)
-        Sg = R @ torch.diag_embed(s * s) @ R.transpose(1, 2)
-        out["cov3D_precomp"] = torch.stack([Sg[:, 0, 0], Sg[:, 0, 1], Sg[:, 0, 2], Sg[:, 1, 1], Sg[:, 1, 2],
-                                            Sg[:, 2, 2]], -1).float().contiguous()
+        out["cov3D_precomp"] = cov3D_of(sc["scales"], sc["rotations"])
         out["shs"] = None; out["scales"] = None; out["rotations"] = None
     else:
         out["shs"] = sc["shs"]; out["scales"] = sc["scales"]; out["rotations"] = sc["rotations"]
