@@ -1,7 +1,7 @@
 """Warp LucidDreamer's generated point cloud into camera views on the device (include/gspcd.h).
 
 `warp_view` replaces the per-pose projection and `griddata` block of `LucidDreamer.generate_pcd`'s dreaming stage,
-`align_frames` the whole aligning stage (every generation pose times every hemisphere view, in one call). Both
+`grow_view` the same stage's growth of the cloud from the inpainted view, `align_frames` the whole aligning stage (every generation pose times every hemisphere view, in one call). Both
 follow the reference's numpy expressions: the projection in float64, `np.where` order of the valid points,
 `np.round` (half to even), linear interpolation in the Delaunay triangulation of the projected points with
 fill value 0, the edge ring, and the 9x9 maximum / 11x11 minimum filters with `mode='reflect'`.
@@ -33,6 +33,9 @@ SYMBOLS = [
                               C.c_uint64, _P]),
     ("gspcd_warp_view", C.c_int, [_P, _P, C.c_int64, _P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P,
                                   C.c_uint64, _P]),
+    ("gspcd_grow_scratch_bytes", C.c_int, [C.c_int64, C.c_int32, C.c_int32, C.POINTER(C.c_uint64)]),
+    ("gspcd_grow_view", C.c_int, [_P, C.c_int64, C.c_int32, _P, _P, _P, C.c_int64, _P, _P, _P, C.c_int32, C.c_int32,
+                                  _P, C.c_int64, _P, _P, _P, _P, _P, _P, _P, C.c_uint64, _P]),
 ]
 
 _lib = None
@@ -184,3 +187,110 @@ def align_frames(pts, colors, render_poses, internal_poses, K, H: int, W: int):
     keep = [k for k in range(V) if small_h[k] > 0]
     out = frames[keep].cpu().numpy() if keep else np.zeros((0, H, W, 3), np.uint8)
     return out, [views[k][2] for k in keep]
+
+
+def grow_matrices(R, T, K) -> np.ndarray:
+    """The 48 host float64 values gspcd_grow_view reads, formed with the reference's own numpy / torch expressions
+    (`generate_pcd`, dreaming stage), so that the device never inverts anything."""
+    invR = np.linalg.inv(R)
+    invR32 = torch.tensor(invR).float()
+    invRT32 = invR32.matmul(torch.tensor(T).float())                  # the torch product of the border points
+    origin = - np.linalg.inv(R).dot(T).astype(np.float32)              # camera_origin_coord_world2
+    parts = [np.linalg.inv(K), invR32.numpy(), invRT32.numpy(), origin, invR, np.linalg.inv(R).dot(T), R, T]
+    return np.ascontiguousarray(np.concatenate([np.asarray(a, np.float64).reshape(-1) for a in parts]))
+
+
+def _as_cuda_exact(a, dtype, dev, name, shape):
+    """A numpy array, PIL image or CUDA tensor of exactly `dtype` and `shape`, on the device."""
+    if isinstance(a, torch.Tensor):
+        if not a.is_cuda:
+            raise TypeError(f"{name} must be a numpy array or a CUDA tensor")
+        t = a
+    else:
+        t = np.asarray(a)
+        if t.dtype == object:
+            raise TypeError(f"{name} must be a numpy array, a PIL image or a CUDA tensor")
+        t = torch.from_numpy(np.array(t))                              # a copy: PIL arrays are read-only
+    if t.dtype != dtype:
+        raise TypeError(f"{name} must be {dtype}, got {t.dtype}")
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError(f"{name} must have shape {tuple(shape)}, got {tuple(t.shape)}")
+    return t.to(dev).contiguous()
+
+
+def grow_view(pts, colors, R, T, K, mask2, valid_idx, pixel_coord, round_coord, image, depth,
+              return_details: bool = False):
+    """The dreaming stage's growth of the cloud from the inpainted view (`generate_pcd` after
+    `depth_curr = self.d(image_curr)`): border points of `mask2`, their depth corrections, linear (then nearest)
+    interpolation of the correction over the pixels where `mask2 != 1`, and their back-projection and colours.
+
+    `pts` [3, N] float32 (the first view's cloud) or float64, `colors` [N, 3] float32; `K` float32, as
+    `CameraParams` makes it; `mask2`, `valid_idx`, `pixel_coord`, `round_coord` as `warp_view` returns them; `image`
+    uint8 [H, W, 3] (numpy, PIL image or CUDA tensor), `depth` float32 [H, W] (numpy or CUDA tensor). Returns the
+    grown cloud as numpy, float64 [3, N + M] and float32 [N + M, 3], the old points copied exactly; with
+    `return_details` also `border_valid_idx` (int64) and the interpolated correction `new_depth` [M] float64.
+
+    The reference's scale fit is not run: `torch.tensor([[sc, ...]])` copies `sc`, so no gradient reaches it and
+    `trans3d` stays the identity."""
+    dev = _device()
+    if getattr(K, "dtype", None) != np.float32:
+        raise TypeError(f"K must be float32 as CameraParams makes it, got {getattr(K, 'dtype', type(K))}")
+    K = np.asarray(K)
+    if K.shape != (3, 3):
+        raise ValueError(f"K must be 3x3, got {K.shape}")
+    R = np.asarray(R, dtype=np.float64).reshape(3, 3)
+    T = np.asarray(T, dtype=np.float64).reshape(3, 1)
+    if isinstance(pts, torch.Tensor) and not pts.is_cuda or isinstance(colors, torch.Tensor) and not colors.is_cuda:
+        raise TypeError("pts and colors must be numpy arrays or CUDA tensors")
+    pts_h = pts.cpu().numpy() if isinstance(pts, torch.Tensor) else np.asarray(pts)
+    cols_h = colors.cpu().numpy() if isinstance(colors, torch.Tensor) else np.asarray(colors)
+    if pts_h.dtype not in (np.float32, np.float64) or pts_h.ndim != 2 or pts_h.shape[0] != 3:
+        raise ValueError(f"pts must be [3, N] float32 or float64, got {pts_h.shape} {pts_h.dtype}")
+    if cols_h.dtype != np.float32 or cols_h.shape != (pts_h.shape[1], 3):
+        raise ValueError(f"colors must be [N, 3] float32 with N = {pts_h.shape[1]}, got {cols_h.shape} {cols_h.dtype}")
+    mask_h = np.asarray(mask2)
+    if mask_h.ndim != 2 or mask_h.dtype.kind not in "iub":
+        raise ValueError(f"mask2 must be an integer [H, W] array, got {mask_h.shape} {mask_h.dtype}")
+    H, W = mask_h.shape
+    valid_h = np.asarray(valid_idx)
+    nv = valid_h.shape[0] if valid_h.ndim == 1 else -1
+    coords_h, rnd_h = np.asarray(pixel_coord), np.asarray(round_coord)
+    if nv < 0 or coords_h.shape != (2, nv) or rnd_h.shape != (2, nv) or coords_h.dtype != np.float64 or \
+            rnd_h.dtype != np.int32 or valid_h.dtype.kind not in "iu":
+        raise ValueError("valid_idx [n], pixel_coord [2, n] float64 and round_coord [2, n] int32 as warp_view "
+                         "returns them are required")
+    n = pts_h.shape[1]
+    if nv and (valid_h.min() < 0 or valid_h.max() >= n or rnd_h[0].min() < 0 or rnd_h[0].max() >= W or
+               rnd_h[1].min() < 0 or rnd_h[1].max() >= H):
+        raise ValueError("valid_idx or round_coord out of range")
+    img = _as_cuda_exact(image, torch.uint8, dev, "image", (H, W, 3))
+    dep = _as_cuda_exact(depth, torch.float32, dev, "depth", (H, W))
+    M = int((mask_h != 1).sum())
+    f32 = pts_h.dtype == np.float32
+    p = torch.from_numpy(np.ascontiguousarray(pts_h)).to(dev)
+    m2 = torch.from_numpy(np.ascontiguousarray(mask_h.astype(np.int32))).to(dev)
+    vi = torch.from_numpy(valid_h.astype(np.int32)).to(dev)
+    co = torch.from_numpy(np.ascontiguousarray(coords_h)).to(dev)
+    rc = torch.from_numpy(np.ascontiguousarray(rnd_h)).to(dev)
+    mats = grow_matrices(R, T, K)
+    b = C.c_uint64()
+    _check(lib().gspcd_grow_scratch_bytes(nv, H, W, C.byref(b)), "gspcd_grow_scratch_bytes")
+    scratch = torch.empty(b.value, dtype=torch.uint8, device=dev)
+    new_pts = torch.empty((3, max(M, 1)), dtype=torch.float64, device=dev)
+    new_cols = torch.empty((max(M, 1), 3), dtype=torch.float32, device=dev)
+    new_depth = torch.empty(max(M, 1), dtype=torch.float64, device=dev)
+    border = torch.empty(max(nv, 1), dtype=torch.int32, device=dev)
+    small = torch.zeros(2, dtype=torch.int32, device=dev)           # n_border, status
+    _check(lib().gspcd_grow_view(p.data_ptr(), n, int(f32), vi.data_ptr(), co.data_ptr(), rc.data_ptr(), nv,
+                                 m2.data_ptr(), dep.data_ptr(), img.data_ptr(), H, W, mats.ctypes.data, M,
+                                 new_pts.data_ptr(), new_cols.data_ptr(), new_depth.data_ptr(), border.data_ptr(),
+                                 small.data_ptr(), small.data_ptr() + 4, scratch.data_ptr(), scratch.numel(),
+                                 _stream(dev)), "gspcd_grow_view")
+    n_border, status = small.cpu().tolist()
+    if status:
+        raise RuntimeError(f"gspcd_grow_view: status {status} (exact predicate precision or walk cap exceeded)")
+    out_pts = np.concatenate((pts_h, new_pts[:, :M].cpu().numpy()), axis=-1)
+    out_cols = np.concatenate((cols_h, new_cols[:M].cpu().numpy()), axis=0)
+    if not return_details:
+        return out_pts, out_cols
+    return out_pts, out_cols, border[:n_border].cpu().numpy().astype(np.int64), new_depth[:M].cpu().numpy()

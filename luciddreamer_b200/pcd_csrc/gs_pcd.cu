@@ -2,7 +2,8 @@
 // edge ring / max-min filter chain on the device. Per view: project and compact the valid points in index order,
 // write the round mask, bin the points into a uniform cell grid (counting sort, ascending index within a cell),
 // filter the mask, locate the Delaunay triangle of every pixel that needs a value, then assemble the frame with
-// the reference's own expressions. No float atomics; every result is independent of thread scheduling.
+// the reference's own expressions. The grow stage (gspcd_grow_view) reuses the grid, hull and locate steps on the
+// border points of a view. No float atomics; every result is independent of thread scheduling.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -266,6 +267,24 @@ __global__ void k_chain(const double* __restrict__ x, const double* __restrict__
 
 __device__ __forceinline__ bool ring0(int x, int y, int W, int H) { return x == 0 || y == 0 || x == W - 1 || y == H - 1; }
 
+// The Delaunay triangle of q and its barycentric weights: v[] are the input indices of its vertices. False when q lies
+// outside the closed hull (pixels outside it take the fill value without a search), or there are fewer than three
+// points, or all are collinear. griddata's linear value is then 0 + l0 * f(v0) + l1 * f(v1) + l2 * f(v2).
+__device__ __forceinline__ bool locate_linear(const pcd::Grid& g, int count, const int* hull, int hull_n, pcd::Pt q,
+                                              int v[3], double l[3], int& st) {
+    pcd::Located t{{-1, -1, -1}};
+    if (pcd::in_hull(g.x, g.y, hull, hull_n, q, st)) t = pcd::locate(g, count, q, st);
+    if (t.v[0] < 0) return false;
+    const pcd::Pt a = {g.x[t.v[0]], g.y[t.v[0]]}, b = {g.x[t.v[1]], g.y[t.v[1]]}, c = {g.x[t.v[2]], g.y[t.v[2]]};
+    const double t00 = a.x - c.x, t01 = b.x - c.x, t10 = a.y - c.y, t11 = b.y - c.y;
+    const double det = t00 * t11 - t01 * t10, qx = q.x - c.x, qy = q.y - c.y;
+    l[0] = (t11 * qx - t01 * qy) / det;
+    l[1] = (t00 * qy - t10 * qx) / det;
+    l[2] = 1.0 - l[0] - l[1];
+    for (int k = 0; k < 3; ++k) v[k] = g.idx[t.v[k]];
+    return true;
+}
+
 // ---- griddata(..., 'linear', fill_value=0) at the pixels whose value reaches the frame: interior pixels under
 // the 9x9 mask, and the clamped neighbour of every masked pixel of the outermost ring.
 __global__ void k_interp(pcd::Grid g, const int* __restrict__ count, const int* __restrict__ hull,
@@ -288,21 +307,11 @@ __global__ void k_interp(pcd::Grid g, const int* __restrict__ count, const int* 
             }
     }
     if (need) {
-        int st = 0;
-        const pcd::Pt q = {(double)x, (double)y};
-        // pixels outside the closed hull take the fill value without a search
-        pcd::Located t{{-1, -1, -1}};
-        if (pcd::in_hull(g.x, g.y, hull, *hull_n, q, st)) t = pcd::locate(g, *count, q, st);
-        if (t.v[0] >= 0) {
-            const pcd::Pt a = {g.x[t.v[0]], g.y[t.v[0]]}, b = {g.x[t.v[1]], g.y[t.v[1]]}, c = {g.x[t.v[2]], g.y[t.v[2]]};
-            const double t00 = a.x - c.x, t01 = b.x - c.x, t10 = a.y - c.y, t11 = b.y - c.y;
-            const double det = t00 * t11 - t01 * t10, qx = q.x - c.x, qy = q.y - c.y;
-            double l[3];
-            l[0] = (t11 * qx - t01 * qy) / det;
-            l[1] = (t00 * qy - t10 * qx) / det;
-            l[2] = 1.0 - l[0] - l[1];
+        int st = 0, v[3];
+        double l[3];
+        if (locate_linear(g, *count, hull, *hull_n, pcd::Pt{(double)x, (double)y}, v, l, st)) {
             for (int k = 0; k < 3; ++k) {
-                const float* col = colors + (int64_t)vidx[g.idx[t.v[k]]] * 3;
+                const float* col = colors + (int64_t)vidx[v[k]] * 3;
                 for (int ch = 0; ch < 3; ++ch) out[ch] = out[ch] + l[k] * (double)col[ch];
             }
         }
@@ -391,23 +400,62 @@ struct ViewOut {
     int32_t* count_out;
 };
 
+// The buffers of one triangulation: the cell grid of the points, the hull candidates and the hull.
+struct TriBufs {
+    int *cell_count, *cell_start, *cursor, *cell_sums, *sidx;
+    double *sx, *sy;
+    int *ext, *cand_count, *cand_start, *cand_sums, *cand_n, *cand, *hull, *hull_n;
+};
+
+// Bins the first *count of the points (cx, cy) (at most n) into the cell grid gd, ascending index within a cell, and
+// builds their convex hull: what locate_linear needs. Shared by the warp and the grow stage.
+pcd::Grid enqueue_triangulate(const double* cx, const double* cy, const int* count, int64_t n, const GridDims& gd,
+                              const TriBufs& b, int32_t* status, cudaStream_t st) {
+    const int ncell = gd.gw * gd.gh;
+    const int T = 256;
+    const int nbp = (int)((n + T - 1) / T);
+    cudaMemsetAsync(b.cell_count, 0, 4 * (size_t)(ncell + 1), st);
+    if (n > 0) k_cell_count<<<nbp, T, 0, st>>>(cx, cy, count, gd, b.cell_count);
+    exclusive_scan(b.cell_count, b.cell_start, ncell + 1, b.cell_sums, nullptr, st);
+    if (n > 0) {
+        cudaMemcpyAsync(b.cursor, b.cell_start, 4 * (size_t)ncell, cudaMemcpyDeviceToDevice, st);
+        k_cell_scatter<<<nbp, T, 0, st>>>(cx, cy, count, gd, b.cursor, b.sidx);
+        k_cell_sort<<<(ncell + T - 1) / T, T, 0, st>>>(b.cell_start, ncell, b.sidx);
+        k_cell_gather<<<nbp, T, 0, st>>>(count, b.sidx, cx, cy, b.sx, b.sy);
+    }
+    int* top = b.ext; int* bot = top + gd.gw; int* left = bot + gd.gw; int* right = left + gd.gh;
+    const int nbc = (ncell + T - 1) / T;
+    cudaMemsetAsync(top, 0xff, 4 * (size_t)gd.gw, st);                // -1
+    cudaMemsetAsync(bot, 0x7f, 4 * (size_t)gd.gw, st);                // larger than any row
+    cudaMemsetAsync(left, 0x7f, 4 * (size_t)gd.gh, st);
+    cudaMemsetAsync(right, 0xff, 4 * (size_t)gd.gh, st);
+    cudaMemsetAsync(b.cand_count + ncell, 0, 4, st);
+    k_extents<<<nbc, T, 0, st>>>(b.cell_start, gd.gw, gd.gh, top, bot, left, right);
+    k_cand_count<<<nbc, T, 0, st>>>(b.cell_start, gd.gw, gd.gh, top, bot, left, right, b.cand_count);
+    exclusive_scan(b.cand_count, b.cand_start, ncell + 1, b.cand_sums, b.cand_n, st);
+    k_cand_gather<<<nbc, T, 0, st>>>(b.cell_start, gd.gw, gd.gh, b.cand_start, b.cand);
+    k_cand_sort<<<(gd.gw + T - 1) / T, T, 0, st>>>(b.cand_start, gd.gw, gd.gh, b.sx, b.sy, b.sidx, b.cand);
+    k_chain<<<1, 1, 0, st>>>(b.sx, b.sy, b.cand, b.cand_n, b.hull, b.hull_n, status);
+    return pcd::Grid{gd.gw, gd.gh, gd.s, gd.inv_s, b.cell_start, b.sx, b.sy, b.sidx};
+}
+
 int enqueue_view(const double* pts, const float* colors, int64_t n, const Cam& cam, int H, int W, char* scratch,
                  const Layout& L, const ViewOut& o, int32_t* status, cudaStream_t st) {
     const GridDims gd = grid_dims(n, H, W);
-    const int ncell = gd.gw * gd.gh;
     const int64_t npix = (int64_t)H * W;
     int* flags = (int*)(scratch + L.flags); int* pos = (int*)(scratch + L.pos); int* sums = (int*)(scratch + L.sums);
     int* count = (int*)(scratch + L.count);
-    int* cell_count = (int*)(scratch + L.cell_count); int* cell_start = (int*)(scratch + L.cell_start);
-    int* cursor = (int*)(scratch + L.cursor); int* cell_sums = (int*)(scratch + L.cell_sums);
-    int* sidx = (int*)(scratch + L.sidx); double* sx = (double*)(scratch + L.sx); double* sy = (double*)(scratch + L.sy);
     uint8_t* mround = (uint8_t*)(scratch + L.mround); uint8_t* mtmp = (uint8_t*)(scratch + L.mtmp);
     uint8_t* m9 = (uint8_t*)(scratch + L.m9);
     double* interp = (double*)(scratch + L.interp); double* img = (double*)(scratch + L.img);
     uint8_t* keep = (uint8_t*)(scratch + L.keep); uint8_t* mask = (uint8_t*)(scratch + L.mask);
+    const TriBufs tb{(int*)(scratch + L.cell_count), (int*)(scratch + L.cell_start), (int*)(scratch + L.cursor),
+                     (int*)(scratch + L.cell_sums), (int*)(scratch + L.sidx), (double*)(scratch + L.sx),
+                     (double*)(scratch + L.sy), (int*)(scratch + L.ext), (int*)(scratch + L.cand_count),
+                     (int*)(scratch + L.cand_start), (int*)(scratch + L.cand_sums), (int*)(scratch + L.cand_n),
+                     (int*)(scratch + L.cand), (int*)(scratch + L.hull), (int*)(scratch + L.hull_n)};
 
     cudaMemsetAsync(mround, 0, npix, st);
-    cudaMemsetAsync(cell_count, 0, 4 * (size_t)(ncell + 1), st);
     cudaMemsetAsync(count, 0, 4, st);
     const int T = 256;
     const int nbp = (int)((n + T - 1) / T);
@@ -415,37 +463,13 @@ int enqueue_view(const double* pts, const float* colors, int64_t n, const Cam& c
         k_flags<<<nbp, T, 0, st>>>(pts, n, cam, W, H, flags);
         exclusive_scan(flags, pos, n, sums, count, st);
         k_compact<<<nbp, T, 0, st>>>(pts, n, cam, W, H, flags, pos, o.vidx, o.cx, o.cy, o.rx, o.ry, mround);
-        k_cell_count<<<nbp, T, 0, st>>>(o.cx, o.cy, count, gd, cell_count);
-    }
-    exclusive_scan(cell_count, cell_start, ncell + 1, cell_sums, nullptr, st);
-    if (n > 0) {
-        cudaMemcpyAsync(cursor, cell_start, 4 * (size_t)ncell, cudaMemcpyDeviceToDevice, st);
-        k_cell_scatter<<<nbp, T, 0, st>>>(o.cx, o.cy, count, gd, cursor, sidx);
-        k_cell_sort<<<(ncell + T - 1) / T, T, 0, st>>>(cell_start, ncell, sidx);
-        k_cell_gather<<<nbp, T, 0, st>>>(count, sidx, o.cx, o.cy, sx, sy);
     }
     if (o.count_out) k_copy_count<<<1, 1, 0, st>>>(count, o.count_out);
     const int nbx = (int)((npix + T - 1) / T);
     k_filter<true, 4, true><<<nbx, T, 0, st>>>(mround, mtmp, W, H);
     k_filter<true, 4, false><<<nbx, T, 0, st>>>(mtmp, m9, W, H);
-    int* top = (int*)(scratch + L.ext); int* bot = top + gd.gw; int* left = bot + gd.gw; int* right = left + gd.gh;
-    int* cand_count = (int*)(scratch + L.cand_count); int* cand_start = (int*)(scratch + L.cand_start);
-    int* cand_sums = (int*)(scratch + L.cand_sums); int* cand_n = (int*)(scratch + L.cand_n);
-    int* cand = (int*)(scratch + L.cand); int* hull = (int*)(scratch + L.hull); int* hull_n = (int*)(scratch + L.hull_n);
-    const int nbc = (ncell + T - 1) / T;
-    cudaMemsetAsync(top, 0xff, 4 * (size_t)gd.gw, st);                // -1
-    cudaMemsetAsync(bot, 0x7f, 4 * (size_t)gd.gw, st);                // larger than any row
-    cudaMemsetAsync(left, 0x7f, 4 * (size_t)gd.gh, st);
-    cudaMemsetAsync(right, 0xff, 4 * (size_t)gd.gh, st);
-    cudaMemsetAsync(cand_count + ncell, 0, 4, st);
-    k_extents<<<nbc, T, 0, st>>>(cell_start, gd.gw, gd.gh, top, bot, left, right);
-    k_cand_count<<<nbc, T, 0, st>>>(cell_start, gd.gw, gd.gh, top, bot, left, right, cand_count);
-    exclusive_scan(cand_count, cand_start, ncell + 1, cand_sums, cand_n, st);
-    k_cand_gather<<<nbc, T, 0, st>>>(cell_start, gd.gw, gd.gh, cand_start, cand);
-    k_cand_sort<<<(gd.gw + T - 1) / T, T, 0, st>>>(cand_start, gd.gw, gd.gh, sx, sy, sidx, cand);
-    k_chain<<<1, 1, 0, st>>>(sx, sy, cand, cand_n, hull, hull_n, status);
-    pcd::Grid g{gd.gw, gd.gh, gd.s, gd.inv_s, cell_start, sx, sy, sidx};
-    k_interp<<<(int)((npix + 127) / 128), 128, 0, st>>>(g, count, hull, hull_n, m9, o.vidx, colors, W, H, interp,
+    const pcd::Grid g = enqueue_triangulate(o.cx, o.cy, count, n, gd, tb, status, st);
+    k_interp<<<(int)((npix + 127) / 128), 128, 0, st>>>(g, count, tb.hull, tb.hull_n, m9, o.vidx, colors, W, H, interp,
                                                          status);
     k_assemble<<<nbx, T, 0, st>>>(interp, m9, W, H, img, keep);
     k_filter<false, 5, true><<<nbx, T, 0, st>>>(keep, mtmp, W, H);
@@ -470,6 +494,198 @@ bool common_args_ok(const double* pts, const float* colors, int64_t n, const dou
     if (!K || !status || !scratch || !aligned(status, 4) || !aligned(scratch, 256)) return false;
     if (n > 0 && (!pts || !colors || !aligned(pts, 8) || !aligned(colors, 4))) return false;
     return scratch_bytes >= layout(n, H, W).total;
+}
+
+// ---- the grow stage (gspcd_grow_view): border points, their depth corrections, griddata linear / nearest over the
+// inpainted pixels, back-projection. Every expression follows the reference's numpy / torch one, with the rounding
+// of the CPU BLAS for a [3x3] @ [3xn] product: fma(a2, b2, fma(a1, b1, a0 * b0)) per row, zero entries included
+// (they decide signed zeros).
+struct GrowMats {
+    float invK[9], invR32[9], invRT32[3], origin[3];                   // float32 quantities of the reference
+    double invK64[9], invR[9], invRT[3], R[9], T[3];
+};
+
+__device__ __forceinline__ float chain32(const float* a, float b0, float b1, float b2) {
+    return __fmaf_rn(a[2], b2, __fmaf_rn(a[1], b1, __fmul_rn(a[0], b0)));
+}
+__device__ __forceinline__ double chain64(const double* a, double b0, double b1, double b2) {
+    return __fma_rn(a[2], b2, __fma_rn(a[1], b1, __dmul_rn(a[0], b0)));
+}
+
+// x86's default NaN, which numpy's invalid operations produce
+__device__ __forceinline__ double nan64() { return __longlong_as_double((long long)0xFFF8000000000000ull); }
+__device__ __forceinline__ float nan32() { return __int_as_float((int)0xFFC00000u); }
+
+// matmul(eye(4), [p; 1])[:3] / [-1], the identity trans3d the scale fit leaves: each coordinate plus zeros (-0.0
+// becomes +0.0), and 0 * inf or 0 * NaN makes a point with any non-finite coordinate NaN throughout.
+__device__ __forceinline__ void identity3d(float p[3]) {
+    const bool fin = isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]);
+    for (int r = 0; r < 3; ++r) p[r] = fin ? __fadd_rn(p[r], 0.0f) : nan32();
+}
+__device__ __forceinline__ void identity3d(double p[3]) {
+    const bool fin = isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]);
+    for (int r = 0; r < 3; ++r) p[r] = fin ? __dadd_rn(p[r], 0.0) : nan64();
+}
+
+// mask_hf at (ry, rx): |m - m(below)| + |m - m(right)| >= 0.3, the last row and column padded from their neighbours
+__global__ void k_border_flags(const int32_t* __restrict__ rnd, int64_t nv, const int32_t* __restrict__ mask2, int W,
+                               int H, int* __restrict__ flags) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= nv) return;
+    const int x = min(rnd[j], W - 2), y = min(rnd[nv + j], H - 2);
+    const int32_t m = mask2[(int64_t)y * W + x];
+    flags[j] = (m != mask2[(int64_t)(y + 1) * W + x] || m != mask2[(int64_t)y * W + x + 1]) ? 1 : 0;
+}
+
+// One border point: the torch float32 back-projection of its round pixel, the ray from the camera origin, the cloud
+// point's projection onto it, and z(R comp + T) - z(R campixel + T). F32: the first view's float32 cloud.
+template <bool F32>
+__global__ void k_border_values(const void* __restrict__ pts_v, int64_t n, const int32_t* __restrict__ valid_idx,
+                                const double* __restrict__ coords, const int32_t* __restrict__ rnd, int64_t nv,
+                                const int* __restrict__ flags, const int* __restrict__ pos,
+                                const float* __restrict__ depth, int W, GrowMats M, double* __restrict__ px,
+                                double* __restrict__ py, double* __restrict__ val, int32_t* __restrict__ border_idx) {
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= nv || !flags[j]) return;
+    const int rx = rnd[j], ry = rnd[nv + j];
+    const float d = depth[(int64_t)ry * W + rx];
+    const float X = __fmul_rn((float)rx, d), Y = __fmul_rn((float)ry, d);
+    float cam[3], cp[3], vc[3];
+    for (int r = 0; r < 3; ++r) cam[r] = chain32(M.invK + 3 * r, X, Y, d);
+    for (int r = 0; r < 3; ++r) cp[r] = __fsub_rn(chain32(M.invR32 + 3 * r, cam[0], cam[1], cam[2]), M.invRT32[r]);
+    identity3d(cp);
+    for (int r = 0; r < 3; ++r) vc[r] = __fsub_rn(cp[r], M.origin[r]);
+    const float den = __fadd_rn(__fadd_rn(__fmul_rn(vc[0], vc[0]), __fmul_rn(vc[1], vc[1])), __fmul_rn(vc[2], vc[2]));
+    const int64_t i = valid_idx[j];
+    double comp[3];
+    if (F32) {
+        const float* pts = (const float*)pts_v;
+        float vp[3];
+        for (int r = 0; r < 3; ++r) vp[r] = __fsub_rn(pts[r * n + i], M.origin[r]);
+        const float num = __fadd_rn(__fadd_rn(__fmul_rn(vp[0], vc[0]), __fmul_rn(vp[1], vc[1])), __fmul_rn(vp[2], vc[2]));
+        const float coeff = __fdiv_rn(num, den);
+        for (int r = 0; r < 3; ++r) comp[r] = (double)__fadd_rn(M.origin[r], __fmul_rn(vc[r], coeff));
+    } else {
+        const double* pts = (const double*)pts_v;
+        double vp[3];
+        for (int r = 0; r < 3; ++r) vp[r] = __dsub_rn(pts[r * n + i], (double)M.origin[r]);
+        const double num = __dadd_rn(__dadd_rn(__dmul_rn(vp[0], (double)vc[0]), __dmul_rn(vp[1], (double)vc[1])),
+                                     __dmul_rn(vp[2], (double)vc[2]));
+        const double coeff = __ddiv_rn(num, (double)den);
+        for (int r = 0; r < 3; ++r) comp[r] = __dadd_rn((double)M.origin[r], __dmul_rn((double)vc[r], coeff));
+    }
+    const double zc = __dadd_rn(chain64(M.R + 6, comp[0], comp[1], comp[2]), M.T[2]);
+    const double zh = __dadd_rn(chain64(M.R + 6, (double)cp[0], (double)cp[1], (double)cp[2]), M.T[2]);
+    const int k = pos[j];
+    px[k] = coords[j];
+    py[k] = coords[nv + j];
+    val[k] = __dsub_rn(zc, zh);
+    if (border_idx) border_idx[k] = (int32_t)j;
+}
+
+// The four image corners with value 0 after the border points, in the reference's order.
+__global__ void k_corners(const int* __restrict__ nb, int W, int H, double* __restrict__ px, double* __restrict__ py,
+                          double* __restrict__ val, int* __restrict__ npts, int32_t* __restrict__ n_border) {
+    const int b = *nb;
+    const double cx[4] = {0.0, 0.0, (double)(W - 1), (double)(W - 1)}, cy[4] = {0.0, (double)(H - 1), 0.0, (double)(H - 1)};
+    for (int k = 0; k < 4; ++k) { px[b + k] = cx[k]; py[b + k] = cy[k]; val[b + k] = 0.0; }
+    *npts = b + 4;
+    *n_border = b;
+}
+
+// np.where(1 - mask2): the pixels whose mask is not 1
+__global__ void k_inpaint_flags(const int32_t* __restrict__ mask2, int64_t npix, int* __restrict__ flags) {
+    const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p < npix) flags[p] = mask2[p] != 1 ? 1 : 0;
+}
+
+// One inpainted pixel: griddata linear over the border points and corners (NaN outside the hull or from a NaN
+// vertex value), nearest where that is NaN, then the back-projection of depth + correction and the colour.
+__global__ void k_grow(pcd::Grid g, const int* __restrict__ npts, const int* __restrict__ hull,
+                       const int* __restrict__ hull_n, const double* __restrict__ val,
+                       const int32_t* __restrict__ mask2, const int* __restrict__ ipos, const float* __restrict__ depth,
+                       const uint8_t* __restrict__ image, int W, int H, GrowMats M, int64_t m_new,
+                       double* __restrict__ new_pts, float* __restrict__ new_colors, double* __restrict__ new_depth,
+                       int* __restrict__ status) {
+    const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= (int64_t)W * H || mask2[p] == 1) return;
+    const int64_t m = ipos[p];
+    if (m >= m_new) return;
+    const int x = (int)(p % W), y = (int)(p / W);
+    const pcd::Pt q = {(double)x, (double)y};
+    int st = 0, v[3];
+    double l[3], nd = nan64();
+    if (locate_linear(g, *npts, hull, *hull_n, q, v, l, st)) {
+        nd = 0.0;
+        for (int k = 0; k < 3; ++k) nd = nd + l[k] * val[v[k]];
+    }
+    if (isnan(nd)) {
+        pcd::NearestQuery nq{&g, q, 0.0, -1, 0};
+        pcd::NearestDone done{&nq};
+        pcd::ring_search(g, q.x, q.y, nq, done);
+        nd = val[g.idx[nq.best]];
+    }
+    if (st) atomicOr(status, st);
+    const float d = depth[p];
+    float pc[3];
+    for (int r = 0; r < 3; ++r) pc[r] = chain32(M.invK + 3 * r, __fmul_rn((float)x, d), __fmul_rn((float)y, d), d);
+    const double X = __dmul_rn((double)x, nd), Y = __dmul_rn((double)y, nd);
+    double s[3], w[3];
+    for (int r = 0; r < 3; ++r) s[r] = __dadd_rn((double)pc[r], chain64(M.invK64 + 3 * r, X, Y, nd));
+    for (int r = 0; r < 3; ++r) w[r] = (double)__double2float_rn(__dsub_rn(chain64(M.invR + 3 * r, s[0], s[1], s[2]), M.invRT[r]));
+    identity3d(w);
+    for (int r = 0; r < 3; ++r) new_pts[r * m_new + m] = w[r];
+    for (int ch = 0; ch < 3; ++ch) new_colors[m * 3 + ch] = __fdiv_rn((float)image[p * 3 + ch], 255.0f);
+    if (new_depth) new_depth[m] = nd;
+}
+
+struct GrowLayout {
+    size_t flags, pos, sums, nb, npts, px, py, val, iflags, ipos, isums;
+    size_t cell_count, cell_start, cursor, cell_sums, sidx, sx, sy, ext, cand_count, cand_start, cand_sums, cand_n,
+        cand, hull, hull_n, total;
+};
+
+// The grid is sized for a border of about four image perimeters; only the search time depends on it.
+GridDims grow_grid(int64_t nv, int H, int W) {
+    const int64_t per = 4 * ((int64_t)H + W);
+    return grid_dims((nv < per ? nv : per) + 4, H, W);
+}
+
+GrowLayout grow_layout(int64_t nv, int H, int W) {
+    const GridDims g = grow_grid(nv, H, W);
+    const int64_t ncell = (int64_t)g.gw * g.gh, npix = (int64_t)H * W, nn = nv > 0 ? nv : 1, np4 = nv + 4;
+    GrowLayout L{};
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t at = o; o = align_up(o + bytes); return at; };
+    L.flags = take(4 * nn); L.pos = take(4 * nn); L.sums = take(4 * (nn / SCAN_BLOCK + 1));
+    L.nb = take(4); L.npts = take(4);
+    L.px = take(8 * np4); L.py = take(8 * np4); L.val = take(8 * np4);
+    L.iflags = take(4 * npix); L.ipos = take(4 * npix); L.isums = take(4 * (npix / SCAN_BLOCK + 1));
+    L.cell_count = take(4 * (ncell + 1)); L.cell_start = take(4 * (ncell + 1)); L.cursor = take(4 * (ncell + 1));
+    L.cell_sums = take(4 * ((ncell + 1) / SCAN_BLOCK + 1));
+    L.sidx = take(4 * np4); L.sx = take(8 * np4); L.sy = take(8 * np4);
+    L.ext = take(8 * ((int64_t)g.gw + g.gh));
+    L.cand_count = take(4 * (ncell + 1)); L.cand_start = take(4 * (ncell + 1));
+    L.cand_sums = take(4 * ((ncell + 1) / SCAN_BLOCK + 1)); L.cand_n = take(4);
+    L.cand = take(4 * np4); L.hull = take(4 * (2 * np4 + 1)); L.hull_n = take(4);
+    L.total = o;
+    return L;
+}
+
+GrowMats grow_mats(const double* m) {
+    GrowMats M;
+    for (int i = 0; i < 9; ++i) { M.invK[i] = (float)m[i]; M.invK64[i] = (double)(float)m[i]; }
+    for (int i = 0; i < 9; ++i) M.invR32[i] = (float)m[9 + i];
+    for (int i = 0; i < 3; ++i) { M.invRT32[i] = (float)m[18 + i]; M.origin[i] = (float)m[21 + i]; }
+    for (int i = 0; i < 9; ++i) M.invR[i] = m[24 + i];
+    for (int i = 0; i < 3; ++i) M.invRT[i] = m[33 + i];
+    for (int i = 0; i < 9; ++i) M.R[i] = m[36 + i];
+    for (int i = 0; i < 3; ++i) M.T[i] = m[45 + i];
+    return M;
+}
+
+bool grow_sizes_ok(int64_t nv, int H, int W) {
+    return nv >= 0 && nv <= (int64_t)INT32_MAX / 2 && H >= 3 && W >= 3 && (int64_t)H * W <= (int64_t)INT32_MAX / 4;
 }
 
 }  // namespace
@@ -524,6 +740,67 @@ int gspcd_warp_view(const double* pts, const float* colors, int64_t n, const dou
               n > 0 ? coords + nn : (double*)(s + L.cy), n > 0 ? round_coords : (int*)(s + L.rx),
               n > 0 ? round_coords + nn : (int*)(s + L.ry), count};
     return enqueue_view(pts, colors, n, make_cam(pose, K), H, W, s, L, o, status, st);
+}
+
+int gspcd_grow_scratch_bytes(int64_t n_valid, int32_t H, int32_t W, uint64_t* bytes) {
+    if (!bytes || !grow_sizes_ok(n_valid, H, W)) return GSPCD_EINVAL;
+    *bytes = grow_layout(n_valid, H, W).total;
+    return GSPCD_OK;
+}
+
+int gspcd_grow_view(const void* pts, int64_t n, int32_t cloud_is_f32, const int32_t* valid_idx, const double* coords,
+                    const int32_t* round_coords, int64_t n_valid, const int32_t* mask2, const float* depth,
+                    const uint8_t* image, int32_t H, int32_t W, const double* mats, int64_t m_new, double* new_pts,
+                    float* new_colors, double* new_depth, int32_t* border_idx, int32_t* n_border, int32_t* status,
+                    void* scratch, uint64_t scratch_bytes, void* stream) {
+    if (!grow_sizes_ok(n_valid, H, W) || n < n_valid || n > (int64_t)INT32_MAX / 2) return GSPCD_EINVAL;
+    if (cloud_is_f32 != 0 && cloud_is_f32 != 1) return GSPCD_EINVAL;
+    if (m_new < 0 || m_new > (int64_t)H * W) return GSPCD_EINVAL;
+    if (!mask2 || !depth || !image || !mats || !new_pts || !new_colors || !n_border || !status || !scratch)
+        return GSPCD_EINVAL;
+    if (!aligned(mask2, 4) || !aligned(depth, 4) || !aligned(new_pts, 8) || !aligned(new_colors, 4) ||
+        !aligned(n_border, 4) || !aligned(status, 4) || !aligned(scratch, 256))
+        return GSPCD_EINVAL;
+    if ((new_depth && !aligned(new_depth, 8)) || (border_idx && !aligned(border_idx, 4))) return GSPCD_EINVAL;
+    if (n_valid > 0 && (!pts || !valid_idx || !coords || !round_coords || !aligned(pts, cloud_is_f32 ? 4 : 8) ||
+                        !aligned(valid_idx, 4) || !aligned(coords, 8) || !aligned(round_coords, 4)))
+        return GSPCD_EINVAL;
+    const GrowLayout L = grow_layout(n_valid, H, W);
+    if (scratch_bytes < L.total) return GSPCD_EINVAL;
+    cudaStream_t st = (cudaStream_t)stream;
+    char* s = (char*)scratch;
+    const GrowMats M = grow_mats(mats);
+    const GridDims gd = grow_grid(n_valid, H, W);
+    const int64_t npix = (int64_t)H * W;
+    int* flags = (int*)(s + L.flags); int* pos = (int*)(s + L.pos); int* nb = (int*)(s + L.nb);
+    int* npts = (int*)(s + L.npts); int* ipos = (int*)(s + L.ipos); int* iflags = (int*)(s + L.iflags);
+    double* px = (double*)(s + L.px); double* py = (double*)(s + L.py); double* val = (double*)(s + L.val);
+    const TriBufs tb{(int*)(s + L.cell_count), (int*)(s + L.cell_start), (int*)(s + L.cursor), (int*)(s + L.cell_sums),
+                     (int*)(s + L.sidx), (double*)(s + L.sx), (double*)(s + L.sy), (int*)(s + L.ext),
+                     (int*)(s + L.cand_count), (int*)(s + L.cand_start), (int*)(s + L.cand_sums), (int*)(s + L.cand_n),
+                     (int*)(s + L.cand), (int*)(s + L.hull), (int*)(s + L.hull_n)};
+    if (cudaMemsetAsync(status, 0, 4, st) != cudaSuccess) return GSPCD_ECUDA;
+    cudaMemsetAsync(nb, 0, 4, st);
+    const int T = 256;
+    const int nbv = (int)((n_valid + T - 1) / T);
+    if (n_valid > 0) {
+        k_border_flags<<<nbv, T, 0, st>>>(round_coords, n_valid, mask2, W, H, flags);
+        exclusive_scan(flags, pos, n_valid, (int*)(s + L.sums), nb, st);
+        if (cloud_is_f32)
+            k_border_values<true><<<nbv, T, 0, st>>>(pts, n, valid_idx, coords, round_coords, n_valid, flags, pos, depth,
+                                                     W, M, px, py, val, border_idx);
+        else
+            k_border_values<false><<<nbv, T, 0, st>>>(pts, n, valid_idx, coords, round_coords, n_valid, flags, pos,
+                                                      depth, W, M, px, py, val, border_idx);
+    }
+    k_corners<<<1, 1, 0, st>>>(nb, W, H, px, py, val, npts, n_border);
+    const int nbx = (int)((npix + T - 1) / T);
+    k_inpaint_flags<<<nbx, T, 0, st>>>(mask2, npix, iflags);
+    exclusive_scan(iflags, ipos, npix, (int*)(s + L.isums), nullptr, st);
+    const pcd::Grid g = enqueue_triangulate(px, py, npts, n_valid + 4, gd, tb, status, st);
+    k_grow<<<(int)((npix + 127) / 128), 128, 0, st>>>(g, npts, tb.hull, tb.hull_n, val, mask2, ipos, depth, image, W, H,
+                                                       M, m_new, new_pts, new_colors, new_depth, status);
+    return cudaPeekAtLastError() == cudaSuccess ? GSPCD_OK : GSPCD_ECUDA;
 }
 
 }  // extern "C"
