@@ -163,11 +163,12 @@ def compose_poses(render_poses, internal_poses):
     return out
 
 
-def align_frames(pts, colors, render_poses, internal_poses, K, H: int, W: int):
+def align_frames(pts, colors, render_poses, internal_poses, K, H: int, W: int, on_device: bool = False):
     """The aligning stage of `generate_pcd`: every generation pose times every hemisphere view, one device call.
 
     Returns (frames [n, H, W, 3] uint8, [Pc2w 4x4 float64] * n), skipping views with no valid point like the
-    reference's `continue`. `frames[k]` is `np.round(imagej*255.).astype(np.uint8)` of the k-th kept view."""
+    reference's `continue`. `frames[k]` is `np.round(imagej*255.).astype(np.uint8)` of the k-th kept view. With
+    `on_device` the frames stay on the device as a uint8 CUDA tensor, ready for `scene.build_scene(frames=...)`."""
     dev = _device()
     p, c = _cloud(pts, colors, dev)
     n = p.shape[1]
@@ -185,7 +186,10 @@ def align_frames(pts, colors, render_poses, internal_poses, K, H: int, W: int):
     if small_h[V]:
         raise RuntimeError(f"gspcd_align: status {small_h[V]} (exact predicate precision or walk cap exceeded)")
     keep = [k for k in range(V) if small_h[k] > 0]
-    out = frames[keep].cpu().numpy() if keep else np.zeros((0, H, W, 3), np.uint8)
+    if on_device:
+        out = frames[:V] if len(keep) == V else frames[keep]
+    else:
+        out = frames[keep].cpu().numpy() if keep else np.zeros((0, H, W, 3), np.uint8)
     return out, [views[k][2] for k in keep]
 
 
