@@ -8,8 +8,9 @@ graph.
     step.check()                                       # raises if a replay overflowed the pair capacity
 
 The graph reads the raw parameters, the optimiser state and gm.xyz_gradient_accum / denom / max_radii2D in place.  The
-reference's densify_and_prune and reset_opacity (scene/gaussian_model.py:210-401) keep running unchanged between
-iterations; they replace those tensors, and the next run() re-captures.  So does a change of gm.active_sh_degree.
+reference's densify_and_prune and reset_opacity (scene/gaussian_model.py:210-401) run between iterations, as they are
+or on the device after densify.attach(gm) (luciddreamer_b200/densify.py, the same results); either replaces those
+tensors, and the next run() re-captures.  So does a change of gm.active_sh_degree.
 
 Iterations that edit the model run with step=False: statistics without the optimiser.  After the edit, step_unchanged()
 steps the groups whose Parameter survived it, which is what the reference's optimizer.step() does (every replaced
