@@ -381,6 +381,12 @@ int gs_debug_export_binning(const GsFrame* f, const void* binning_buffer, int64_
                             const void* image_buffer, uint32_t* tile_offsets, uint32_t* point_list,
                             int64_t max_pairs, gs_stream_t stream);
 
+/* Introspection for tests: the image rows a warp of the tile passes (forward blend, backward, deterministic partials)
+ * owns when a W x H frame is rendered on ctx's device: 4 (16x4 strips, four warps per tile) or 8 (16x8 blocks, two
+ * warps).  The choice depends on the tile count and the device's SM count; this asks the launch code itself.
+ * Negative on a bad argument. */
+int gs_debug_blend_rows_per_warp(GsContext* ctx, int32_t W, int32_t H);
+
 /* Per-kernel timing for bench.py's roofline leg (no reference counterpart: the reference has no profiling hooks,
  * SURVEY.md section 5).  When enabled, every kernel launch is bracketed by CUDA events on the launching stream;
  * gs_profile_read waits for them and returns the duration in ms of each kernel of the most recent forward /

@@ -122,6 +122,7 @@ SYMBOLS = [
                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("gs_debug_export_binning", C.c_int, [C.POINTER(GsFrame), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_int64, C.c_void_p]),
+    ("gs_debug_blend_rows_per_warp", C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     ("gs_profile_enable", C.c_int, [C.c_void_p, C.c_int]),
     ("gs_profile_num_kernels", C.c_int, []),
     ("gs_profile_kernel_name", C.c_char_p, [C.c_int]),

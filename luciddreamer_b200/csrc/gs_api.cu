@@ -877,4 +877,12 @@ int gs_debug_export_binning(const GsFrame* f, const void* binning_buffer, int64_
     return GS_OK;
 }
 
+int gs_debug_blend_rows_per_warp(GsContext* ctx, int32_t W, int32_t H) {
+    if (!ctx || W <= 0 || H <= 0) return fail(GS_EINVAL, "bad argument");
+    GsView v{};
+    v.W = W; v.H = H;
+    v.gx = (W + GS_TILE - 1) / GS_TILE; v.gy = (H + GS_TILE - 1) / GS_TILE;
+    return gs_blend_use_strips(v) ? 4 : 8;
+}
+
 }  // extern "C"

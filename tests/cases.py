@@ -52,7 +52,26 @@ EXTRA_CASES = [
     Case("frustum_20k_96", 20_000, 96, 96, 3, 23, golden=False, scene="frustum"),
     Case("frustum_60k_64_bg", 60_000, 64, 64, 1, 24, bg=(0.2, 0.5, 0.1), opacity_shift=1.0, golden=False, scene="frustum"),
 ]
-CASES_ALL = CASES + EXTRA_CASES
+# oracle-only cases in the 16x8-block geometry of the tile passes (csrc/gs_blend.cuh: chosen from the tile count and the
+# SM count; 1 500 tiles and more are blocks on every H100 variant, and the GPU tests ask the library which one ran).
+# Between them they reach, in blocks, what EXTRA_CASES reach in strips; both image sides are ragged (not multiples of
+# 16, and H % 8 != 0: the bottom warp of the last tile row holds live and dead rows).
+BLOCK_CASES = [
+    # the plain path: W % 16 = 1, H % 16 = 3
+    Case("blk_shell_60k_721x531_bg", 60_000, 721, 531, 3, 31, scale_mult=2.0, bg=(0.3, 0.6, 0.9), golden=False),
+    # a third of the opacities above the 0.99 clamp, thick stacks: termination on most pixels, whole threads on the
+    # generic path, warps and tiles that leave their lists early
+    Case("blk_opaque_150k_650x615_x6", 150_000, 650, 615, 3, 32, scale_mult=6.0, opacity_shift=4.0, golden=False),
+    # needles: ill-conditioned conics, tile rectangles of hundreds of tiles (hit decisions recomputed per tile)
+    Case("blk_needles_3k_599x685", 3000, 599, 685, 2, 33, scale_mult=3.0, aniso_sigma=2.5, golden=False),
+    # LucidDreamer-shaped and dense (every Gaussian visible); splats of ~12 px sigma, so that 80 000 Gaussians give
+    # per-tile lists on both sides of the 2 048-entry sort size (the same density at 1.5 px sigma would take millions)
+    Case("blk_frustum_80k_633x613_x8", 80_000, 633, 613, 3, 36, scale_mult=8.0, opacity_shift=1.0, golden=False,
+         scene="frustum"),
+    Case("blk_precomp_40k_811x470_bg", 40_000, 811, 470, 0, 35, scale_mult=2.0, bg=(0.1, 0.0, 0.2), scale_modifier=1.7,
+         precomp=True, golden=False),
+]
+CASES_ALL = CASES + EXTRA_CASES + BLOCK_CASES
 BY_NAME = {c.name: c for c in CASES_ALL}
 
 
@@ -71,7 +90,7 @@ def cov3D_of(scales: torch.Tensor, rotations: torch.Tensor) -> torch.Tensor:
 def build_inputs(case: Case) -> Dict[str, object]:
     """CPU float32 tensors + camera in the reference binding's vocabulary."""
     if case.scene == "frustum":
-        sc = syn.make_frustum_scene(case.P, case.seed, case.W, case.H, sigma_px=1.5)
+        sc = syn.make_frustum_scene(case.P, case.seed, case.W, case.H, sigma_px=1.5 * case.scale_mult)
         if case.opacity_shift:
             sc["opacities"] = torch.sigmoid(torch.logit(sc["opacities"]) + case.opacity_shift).contiguous()
     else:

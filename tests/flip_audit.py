@@ -48,6 +48,13 @@ def pixel_margins(fwd, x: int, y: int):
     return m
 
 
+def near_thresholds(m, rel_margin=2e-5):
+    """The kinds of branch whose operand, in the margins `m` of pixel_margins, sits within `rel_margin` of its threshold."""
+    # T accumulates one rounding per contributing splat, hence the wider margin on the termination test
+    return [k for k, lim in (("alpha", rel_margin), ("power", rel_margin), ("T", 50 * rel_margin), ("acc", rel_margin))
+            if m[k] < lim]
+
+
 def explain_outliers(fwd, color, depth, ref_color, ref_depth, tol=1e-4, rel_margin=2e-5, max_pixels=64):
     """Returns (explained, unexplained): lists of (x, y, err_colour, err_depth, kind / margins) for every pixel whose
     colour or depth differs from the reference by more than `tol`."""
@@ -58,9 +65,7 @@ def explain_outliers(fwd, color, depth, ref_color, ref_depth, tol=1e-4, rel_marg
     explained, unexplained = [], []
     for y, x in list(zip(ys.tolist(), xs.tolist()))[:max_pixels]:
         m = pixel_margins(fwd, x, y)
-        # T accumulates one rounding per contributing splat, hence the wider margin on the termination test
-        near = [k for k, lim in (("alpha", rel_margin), ("power", rel_margin), ("T", 50 * rel_margin), ("acc", rel_margin))
-                if m[k] < lim]
+        near = near_thresholds(m, rel_margin)
         rec = (x, y, float(dc[y, x]), float(dd[y, x]), near or {k: float(v) for k, v in m.items() if k in ("alpha", "power", "T", "acc")})
         (explained if near else unexplained).append(rec)
     return explained, unexplained

@@ -132,16 +132,28 @@ def test_autograd_entry_is_bit_reproducible_and_forward_unchanged(case):
         assert rel(runs[0][k], default[k]) <= 1e-5, (case.name, k)
 
 
-@pytest.mark.parametrize("name", ["opaque_40k_64_x8", "frustum_20k_96", "frustum_60k_64_bg"])
+@pytest.mark.parametrize("name", ["opaque_40k_64_x8", "frustum_20k_96", "frustum_60k_64_bg"] + [c.name for c in cases.BLOCK_CASES])
 def test_matches_cpu_oracle(name):
+    """Behind strip partials (k_tile_partials<1>) and, for cases.BLOCK_CASES, behind block partials (k_tile_partials<2>)."""
     from oracle import oracle
     case = cases.BY_NAME[name]
+    if case in cases.BLOCK_CASES:
+        assert util.blend_rows_per_warp(case.W, case.H) == 8
     inp = cases.build_inputs(case)
     f = oracle.rasterize_gaussians(*cases.binding_args(inp))
     og = dict(zip(cases.GRAD_NAMES, oracle.rasterize_gaussians_backward(f, inp["cot"].numpy())[:8]))
     color, radii, depth, leaves = autograd_forward(cases.binding_args(inp, dev()), True)
-    g = autograd_grads(color, leaves, inp["cot"].to(dev()))
-    util.assert_grads_close({AG_NAMES[k]: v.cpu().numpy() for k, v in g.items()}, og, names=grad_names(case), what=name)
+    g = {AG_NAMES[k]: v.cpu().numpy() for k, v in autograd_grads(color, leaves, inp["cot"].to(dev())).items()}
+    if "needles" in name:
+        # beyond fp32 conditioning (test_parity_gpu._check_ill_conditioned): the fp64 oracle is the bar and the fp32
+        # oracle's own distance from it the yardstick
+        t = oracle.rasterize_gaussians(*cases.binding_args(inp)[:17], mode="f64")
+        og64 = dict(zip(cases.GRAD_NAMES, oracle.rasterize_gaussians_backward(t, inp["cot"].numpy())[:8]))
+        for k in grad_names(case) & g.keys():
+            e_ref, e_our = util.rel_err(og[k], og64[k]), util.rel_err(g[k].reshape(og64[k].shape), og64[k])
+            assert e_our <= max(util.GRAD_REL_TOL, 10 * e_ref), f"{name}: {k} rel err {e_our:.3e} vs fp64 (fp32 oracle: {e_ref:.3e})"
+        return
+    util.assert_grads_close(g, og, names=grad_names(case), what=name)
 
 
 def _full_size(kind):

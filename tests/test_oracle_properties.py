@@ -190,21 +190,46 @@ def test_flip_audit_replay_is_faithful():
     raise AssertionError("no wide-margin pixel found")
 
 
-@pytest.mark.parametrize("name", [c.name for c in cases.EXTRA_CASES])
+@pytest.mark.parametrize("name", [c.name for c in cases.EXTRA_CASES + cases.BLOCK_CASES])
 def test_extra_cases_reach_their_branches(name):
     """The oracle-only cases exist to reach early termination, the 0.99 clamp, ill-conditioned conics and long
-    tile lists; make sure the scenes really do (otherwise the GPU parity tests on them prove nothing)."""
+    tile lists, the block cases to reach them on a grid of 1 500 tiles or more with ragged sides; make sure the scenes
+    really do (otherwise the GPU parity tests on them prove nothing)."""
     case = cases.BY_NAME[name]
     inp = cases.build_inputs(case)
     f = _fwd(inp, "f32")
-    rg = f.ranges
-    longest = int((rg[:, 1].astype(np.int64) - rg[:, 0].astype(np.int64)).max())
+    rg = f.ranges.astype(np.int64)
+    lens = rg[:, 1] - rg[:, 0]
+    longest = int(lens.max())
     terminated = float((f.final_T < 1e-3).mean())
-    if name.startswith("opaque"):
-        assert terminated > 0.5 and float((inp["opacities"] > 0.99).float().mean()) > 0.2
+    clamped = float((inp["opacities"] > 0.99).float().mean())
+    visible = float((f.radii > 0).mean())
+    rect = int(f.tiles_touched.max())
+    co = f.geom("conic_opacity", 4)[f.radii > 0].astype(np.float64)
+    det, tr = co[:, 0] * co[:, 2] - co[:, 1] ** 2, co[:, 0] + co[:, 2]
+    ill = float((det < 1e-5 * tr * tr).mean())                 # the blend kernels' conditioning test routes these
+    print(f"{name}: {len(lens)} tiles, terminated {terminated:.3f}, above the clamp {clamped:.3f}, ill-conditioned {ill:.3f}, "
+          f"longest list {longest}, largest rect {rect} tiles, visible {visible:.3f}")
+    if case in cases.BLOCK_CASES:
+        assert len(lens) >= 1500 and case.W % 16 and case.H % 8
+        assert (f.tiles_touched > 32).sum() > 100              # rects beyond the 32-bit hit mask: decisions recomputed
+        full = f.n_contrib[:case.H // 16 * 16, :case.W // 16 * 16] > 0
+        assert (f.n_contrib[case.H // 16 * 16:] > 0).any() and (f.n_contrib[:, case.W // 16 * 16:] > 0).any() and full.any()
+    if name.startswith("blk_shell") or name.startswith("blk_precomp"):
+        assert terminated < 0.01 and visible < 0.1 and (f.radii > 0).sum() > 1000     # the plain, sparse path
+        assert any(case.bg) and (f.final_T > 0.1).mean() > 0.05                         # background shows through
+    elif name.startswith("blk_opaque"):
+        assert terminated > 0.9 and clamped > 0.3 and longest > 256
+    elif name.startswith("blk_needles"):
+        assert ill > 0.05 and rect > 1000 and longest > 256
+    elif name.startswith("blk_frustum"):
+        # dense regime (more than half of the Gaussians visible), lists on both sides of the 2 048-entry sort size with
+        # room for the exact tile culling of the CUDA path, termination
+        assert visible > 0.5 and terminated > 0.9 and lens.min() > 256
+        assert (lens > 3000).sum() >= 10 and (lens < 1800).sum() >= 10
+    elif name.startswith("opaque"):
+        assert terminated > 0.5 and clamped > 0.2
     elif name.startswith("needles"):
-        co = f.geom("conic_opacity", 4)[f.radii > 0].astype(np.float64)
-        det, tr = co[:, 0] * co[:, 2] - co[:, 1] ** 2, co[:, 0] + co[:, 2]
-        assert (det < 1e-5 * tr * tr).mean() > 0.02          # the blend kernels' conditioning test routes these
+        assert ill > 0.02
     else:
         assert terminated > 0.5 and longest > 1500

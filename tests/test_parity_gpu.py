@@ -100,21 +100,24 @@ def image_state(r, H, W):
     return fT, nc
 
 
-ORACLE_CASES = GOLDEN[:6] + cases.EXTRA_CASES
+ORACLE_CASES = GOLDEN[:6] + cases.EXTRA_CASES + cases.BLOCK_CASES
 
 
 @pytest.mark.parametrize("case,entry", by_entry(ORACLE_CASES, [c.name for c in ORACLE_CASES]))
 def test_cuda_matches_cpu_oracle(case, entry):
     """Against the oracle on the same inputs, incl. the oracle-only scenes that reach early termination, the 0.99
-    clamp, ill-conditioned conics (generic blend path) and tile lists beyond every shared-memory sort size."""
+    clamp, ill-conditioned conics (generic blend path) and tile lists beyond every shared-memory sort size, in both
+    geometries of the tile passes (cases.BLOCK_CASES: 16x8 blocks, asked of the library, not assumed)."""
     from oracle import oracle
     inp = cases.build_inputs(case)
     f = oracle.rasterize_gaussians(*cases.binding_args(inp))
     og = dict(zip(cases.GRAD_NAMES, oracle.rasterize_gaussians_backward(f, inp["cot"].numpy())[:8]))
     r = run(entry, cases.binding_args(inp, dev()), inp["cot"])
+    if case in cases.BLOCK_CASES:
+        assert util.blend_rows_per_warp(case.W, case.H) == 8
     if entry == "C":
         assert r["num_rendered"] == f.num_rendered
-    if case.name.startswith("needles"):
+    if "needles" in case.name:
         # Beyond fp32 conditioning: det(cov2D) and `power` lose 3-4 digits to cancellation for needle-shaped splats, so
         # ANY two float32 evaluation orders disagree -- the reference-faithful fp32 oracle itself is off the fp64 oracle
         # by 2e-3 on ~6 % of these pixels (the reference binary, contracted differently by nvcc, would be too).  The bar
@@ -248,39 +251,14 @@ def test_mark_visible():
 def test_binning_order_of_the_C_forward_matches_oracle():
     """Integer pipeline, bit-exact: per-tile lists of the CUDA path are the oracle's lists minus pairs that cannot
     contribute (exact tile culling), in the same (depth, index) order."""
-    import ctypes as C
-    from luciddreamer_b200 import _native as N
     from luciddreamer_b200 import rasterizer as R
     from oracle import oracle
     case = cases.BY_NAME["stress_4k_96_x6"]
     inp = cases.build_inputs(case)
-    d = dev()
     f = oracle.rasterize_gaussians(*cases.binding_args(inp))
-    nr, color, depth, radii, geom, binning, img = R._C.rasterize_gaussians(*cases.binding_args(inp, d))
+    nr, color, depth, radii, geom, binning, img = R._C.rasterize_gaussians(*cases.binding_args(inp, dev()))
     assert nr == f.num_rendered
-    cap = binning.numel() // 12
-    G = ((case.W + 15) // 16) * ((case.H + 15) // 16)
-    off = torch.empty(G + 1, dtype=torch.int32, device=d)
-    lst = torch.empty(cap, dtype=torch.int32, device=d)
-    frame = N.GsFrame()
-    frame.W, frame.H = case.W, case.H
-    N.check(N.lib().gs_debug_export_binning(C.byref(frame), binning.data_ptr(), cap, img.data_ptr(), off.data_ptr(),
-                                            lst.data_ptr(), cap, torch.cuda.current_stream().cuda_stream))
-    torch.cuda.synchronize()
-    off = off.cpu().numpy().astype(np.int64); lst = lst.cpu().numpy().astype(np.int64)
-    assert off[-1] <= nr
-    opl, orng = f.point_list.astype(np.int64), f.ranges.astype(np.int64)
-    depths = f.geom("depths", 1)[:, 0]
-    for t in range(G):
-        mine = lst[off[t]:off[t + 1]]
-        ref = opl[orng[t, 0]:orng[t, 1]]
-        assert set(mine) <= set(ref)
-        # same relative order as the reference list
-        pos = {g: i for i, g in enumerate(ref)}
-        idx = [pos[g] for g in mine]
-        assert idx == sorted(idx)
-        key = [(depths[g], g) for g in mine]
-        assert key == sorted(key)
+    util.assert_binning_matches_oracle(f, case.W, case.H, binning, img)
 
 
 def test_capacity_growth_and_many_views_in_flight():

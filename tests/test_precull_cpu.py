@@ -97,7 +97,7 @@ def test_precull_never_rejects_what_the_reference_keeps(case):
         assert rej > 0.7 * inv, f"{case.name}: only {rej} of {inv} off-screen Gaussians rejected -- the bound is too loose to pay"
 
 
-@pytest.mark.parametrize("case", cases.EXTRA_CASES, ids=lambda c: c.name)
+@pytest.mark.parametrize("case", cases.EXTRA_CASES + cases.BLOCK_CASES, ids=lambda c: c.name)
 def test_precull_never_rejects_what_the_oracle_keeps(case):
     inp = cases.build_inputs(case)
     f = oracle.rasterize_gaussians(*cases.binding_args(inp))

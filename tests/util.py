@@ -53,6 +53,57 @@ def assert_forward_close(color, depth, radii, gold, what="", audit=None, flip_di
                 radii_mismatch=mism)
 
 
+def blend_rows_per_warp(W, H, device_index=0):
+    """Image rows per warp of the tile passes for a W x H frame on this device, as the library's launch code decides it:
+    4 (16x4 strips) or 8 (16x8 blocks)."""
+    from luciddreamer_b200 import _native as N
+    from luciddreamer_b200 import rasterizer as R
+    rows = N.lib().gs_debug_blend_rows_per_warp(R._ctx(device_index), W, H)
+    assert rows in (4, 8), N.last_error()
+    print(f"[geometry] {W}x{H}: {rows} rows per warp")
+    return rows
+
+
+def assert_binning_matches_oracle(f, W, H, binning, img, num_pairs=None):
+    """Integer pipeline of one `_C` forward (its opaque `binning` / `img` buffers), bit-exact against the oracle's forward
+    state `f`: the tile offsets are monotone and end at the device's pair count (when given), and every tile's list is
+    the oracle's list minus pairs that cannot contribute (exact tile culling), in the same (depth, index) order.
+    Returns the device's per-tile list lengths."""
+    import ctypes as C
+
+    import torch
+    from luciddreamer_b200 import _native as N
+    cap = binning.numel() // 12
+    G = ((W + 15) // 16) * ((H + 15) // 16)
+    off = torch.empty(G + 1, dtype=torch.int32, device=binning.device)
+    lst = torch.empty(cap, dtype=torch.int32, device=binning.device)
+    frame = N.GsFrame()
+    frame.W, frame.H = W, H
+    N.check(N.lib().gs_debug_export_binning(C.byref(frame), binning.data_ptr(), cap, img.data_ptr(), off.data_ptr(),
+                                            lst.data_ptr(), cap, torch.cuda.current_stream().cuda_stream))
+    torch.cuda.synchronize()
+    off = off.cpu().numpy().astype(np.int64); lst = lst.cpu().numpy().astype(np.int64)
+    assert off[0] == 0 and np.all(np.diff(off) >= 0), "tile offsets are not monotone"
+    assert off[-1] <= f.num_rendered
+    if num_pairs is not None:
+        assert off[-1] == num_pairs, f"off[G] = {off[-1]}, the device counted {num_pairs} pairs"
+    opl, orng = f.point_list.astype(np.int64), f.ranges.astype(np.int64)
+    depths = f.geom("depths", 1)[:, 0]
+    for t in range(G):
+        mine = lst[off[t]:off[t + 1]]
+        ref = opl[orng[t, 0]:orng[t, 1]]
+        if len(mine) == 0:
+            continue
+        assert set(mine) <= set(ref), f"tile {t}: a Gaussian the oracle does not bin there"
+        # same relative order as the reference list
+        pos = {g: i for i, g in enumerate(ref)}
+        idx = [pos[g] for g in mine]
+        assert idx == sorted(idx), f"tile {t}: order differs from the oracle's list"
+        key = [(depths[g], g) for g in mine]
+        assert key == sorted(key), f"tile {t}: not in (depth, index) order"
+    return np.diff(off)
+
+
 def assert_grads_close(grads, gold_grads, names=None, tol=GRAD_REL_TOL, what=""):
     out = {}
     for k, g in grads.items():
